@@ -8,12 +8,12 @@ from __future__ import annotations
 
 import ctypes as C
 
-SNN_ABI_VERSION = 9
+SNN_ABI_VERSION = 10
 SNN_MAX_LAYERS = 8
 SNN_MAX_CONNS = 12
 
 SNN_NODE_INPUT, SNN_NODE_LIF, SNN_NODE_DC, SNN_NODE_IF, SNN_NODE_CURRENT_LIF, SNN_NODE_BOOSTED_LIF, SNN_NODE_MCP = 0, 1, 2, 3, 4, 5, 6
-SNN_CONN_DENSE, SNN_CONN_MCC, SNN_CONN_CONV2D = 0, 1, 2
+SNN_CONN_DENSE, SNN_CONN_MCC, SNN_CONN_CONV2D, SNN_CONN_SPARSE = 0, 1, 2, 3
 SNN_RULE_NONE, SNN_RULE_NOOP, SNN_RULE_POSTPRE, SNN_RULE_WDEP_POSTPRE, SNN_RULE_MCC_POSTPRE, SNN_RULE_MSTDP, SNN_RULE_HEBBIAN = 0, 1, 2, 3, 4, 5, 6
 SNN_RULE_MSTDPET = 7
 SNN_REDUCE_SUM, SNN_REDUCE_MEAN = 0, 1
@@ -127,6 +127,9 @@ class SnnConn(C.Structure):
         ("e_trace_decay", C.c_float),
         ("tc_e_trace", C.c_float),
         ("et_coef", C.c_float),
+        ("sp_rowptr", C.c_void_p),
+        ("sp_col", C.c_void_p),
+        ("nnz", C.c_int32),
     ]
 
 

@@ -38,10 +38,17 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
     if ((o->delta_w || o->delta_theta) && (o->normalize || !net->learning || o->one_step)) return SNN_ERR_UNSUPPORTED;
     for (int c = 0; c < net->n_conns; ++c) {
         const snn_conn_t &C = net->conns[c];
-        if (C.src < 0 || C.src >= net->n_layers || C.tgt < 0 || C.tgt >= net->n_layers || !C.w) return SNN_ERR_BAD_ARG;
+        const bool sparse = C.kind == SNN_CONN_SPARSE;
+        if (C.src < 0 || C.src >= net->n_layers || C.tgt < 0 || C.tgt >= net->n_layers) return SNN_ERR_BAD_ARG;
+        if (!C.w && !(sparse && C.nnz == 0)) return SNN_ERR_BAD_ARG;
         if (net->layers[C.tgt].kind == SNN_NODE_INPUT) return SNN_ERR_UNSUPPORTED;
         if (C.rule < SNN_RULE_NONE || C.rule > SNN_RULE_MSTDPET) return SNN_ERR_UNSUPPORTED;
-        if (C.kind < SNN_CONN_DENSE || C.kind > SNN_CONN_CONV2D) return SNN_ERR_UNSUPPORTED;
+        if (C.kind < SNN_CONN_DENSE || C.kind > SNN_CONN_SPARSE) return SNN_ERR_UNSUPPORTED;
+        if (sparse) {   // a fixed pattern: static or NoOp-decayed values, no normalize, no mask (snn_b200.h)
+            if (C.rule != SNN_RULE_NONE && C.rule != SNN_RULE_NOOP) return SNN_ERR_UNSUPPORTED;
+            if (C.has_norm || C.mask) return SNN_ERR_UNSUPPORTED;
+            if (C.nnz < 0 || !C.sp_rowptr || (C.nnz > 0 && !C.sp_col)) return SNN_ERR_BAD_ARG;
+        }
         if (C.kind == SNN_CONN_CONV2D) {
             const snn_layer_t &S = net->layers[C.src], &G = net->layers[C.tgt];
             if (C.cin * C.hin * C.win != S.n || C.cout * C.hout * C.wout != G.n || !C.b) return SNN_ERR_BAD_ARG;
@@ -64,6 +71,12 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
         if (C.mask && (C.kind != SNN_CONN_DENSE || SNN_RULE_IS_MSTDP(C.rule))) return SNN_ERR_UNSUPPORTED;
     }
     return SNN_OK;
+}
+
+static bool has_sparse(const snn_net_t *net) {
+    for (int c = 0; c < net->n_conns; ++c)
+        if (net->conns[c].kind == SNN_CONN_SPARSE) return true;
+    return false;
 }
 
 static bool layer_needs_xpub(const snn_net_t *net, int l) {
@@ -126,6 +139,17 @@ static size_t layout_generic(const snn_net_t *net, const snn_run_opts_t *o, char
             if (N) { N->mst[c].sp[0] = C.mst_spre; N->mst[c].st[0] = C.mst_spost; N->mst[c].sp[1] = (uint8_t *)sp; N->mst[c].st[1] = (uint8_t *)st; }
         }
     }
+    // SparseConnections: the column-block offset table of the pattern and the gathered input of the current step
+    for (int c = 0; c < net->n_conns; ++c) {
+        const snn_conn_t &C = net->conns[c];
+        if (C.kind != SNN_CONN_SPARSE) continue;
+        const size_t ns = (size_t)net->layers[C.src].n, nt = (size_t)net->layers[C.tgt].n;
+        const int bw = sparse_block_width((int)ns, (int)nt, o->B, C.nnz), nb = ((int)nt + bw - 1) / bw;
+        if (N) { N->sp[c].bw = bw; N->sp[c].nb = nb; N->sp[c].off = (int32_t *)(ws + off); }
+        off += align_up(sizeof(int32_t) * ns * (size_t)(nb + 1));
+        if (N) N->sp[c].out = (float *)(ws + off);
+        off += align_up(sizeof(float) * B * nt);
+    }
     return off;
 }
 
@@ -134,13 +158,15 @@ extern "C" {
 int snn_b200_abi_version(void) { return SNN_ABI_VERSION; }
 
 const char *snn_b200_build_info(void) {
-    return "libsnn_b200 sm_90a (generic window + fused DC2015 windows v1/v2), ABI " "9" ", built " __DATE__ " " __TIME__;
+    return "libsnn_b200 sm_90a (generic window + fused DC2015 windows v1/v2), ABI " "10" ", built " __DATE__ " " __TIME__;
 }
 
 int snn_b200_last_launch_count(void) { return g_last_launches; }
 
 int snn_b200_select_tier(const snn_net_t *net, const snn_run_opts_t *opts) {
     if (validate(net, opts) != SNN_OK) return 0;
+    if (has_sparse(net))   // the fused DiehlAndCook2015 kernels (and so the delta windows) have no sparse gather
+        return (opts->tier == 0 || opts->tier == 1) && !opts->delta_w && !opts->delta_theta ? 1 : 0;
     if (opts->delta_w || opts->delta_theta)   // delta windows exist in the barrier kernel only
         return (opts->tier == 0 || opts->tier == 2) && snn_fused_dc_supported(net, opts) ? 2 : 0;
     if (opts->tier == 1) return 1;
@@ -156,6 +182,7 @@ int snn_b200_select_tier(const snn_net_t *net, const snn_run_opts_t *opts) {
 size_t snn_b200_workspace_bytes(const snn_net_t *net, const snn_run_opts_t *opts) {
     if (validate(net, opts) != SNN_OK) return 0;
     size_t g = layout_generic(net, opts, nullptr, nullptr);
+    if (has_sparse(net)) return g;
     size_t f = snn_fused_dc_supported(net, opts) ? snn_fused_dc_workspace_bytes(net, opts) : 0;
     size_t f2 = snn_fused_dc2_supported(net, opts) ? snn_fused_dc2_workspace_bytes(net, opts) : 0;
     if (f2 > f) f = f2;

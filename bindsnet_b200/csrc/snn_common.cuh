@@ -56,6 +56,30 @@ struct DevMstdp {
     uint8_t *sp[2], *st[2];
 };
 
+// A SparseConnection (SNN_CONN_SPARSE) in the generic window: its target columns are cut into blocks of `bw` columns;
+// off[i * (nb + 1) + k] is the first CSR position of row i whose column is >= k * bw (k = nb: the row's end), built
+// from the pattern once per window; out holds the connection's gathered input of the current step.
+struct DevSparse {
+    int32_t *off;               // [n_src][nb + 1]
+    float *out;                 // [B][n_tgt]
+    int32_t bw, nb;             // columns per block, blocks
+    int32_t first;              // first gather unit of this connection
+};
+
+// Columns per block of a sparse connection's gather: 1024 (the per-warp accumulator in shared memory) unless the
+// (block, 8-sample chunk) units would leave most of a 132-SM grid idle.  A unit's cost is set by the spiking rows it
+// visits, not by the block width (each spiking row is visited once per block), so blocks are only narrowed until
+// there are about 200 units; never below 128 columns, and never so narrow that the offset table (n_src x (blocks + 1)
+// int32) outgrows max(16 MiB, twice the CSR itself).
+__host__ __device__ inline int sparse_block_width(int n_src, int n_tgt, int B, int nnz) {
+    const double cap = 16.0 * nnz > 16777216.0 ? 16.0 * nnz : 16777216.0;
+    int bw = 1024;
+    while (bw > 128 && (long long)((n_tgt + bw - 1) / bw) * ((B + 7) / 8) < 200 &&
+           4.0 * n_src * ((n_tgt + bw / 2 - 1) / (bw / 2) + 1) <= cap)
+        bw >>= 1;
+    return bw;
+}
+
 struct DevNet {
     int32_t n_layers, n_conns, learning, T, B, normalize, total_items, any_one_spike;
     int32_t any_mask;             // some connection carries a mask (Network.run(..., masks=...))
@@ -70,6 +94,8 @@ struct DevNet {
     DevLayer layers[SNN_MAX_LAYERS];
     snn_conn_t conns[SNN_MAX_CONNS];
     DevMstdp mst[SNN_MAX_CONNS];
+    int32_t sp_units;             // sparse gather units of a step (0: the plan has no SparseConnection)
+    DevSparse sp[SNN_MAX_CONNS];
 };
 
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p) {

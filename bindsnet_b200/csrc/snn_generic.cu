@@ -1,5 +1,5 @@
 // snn_generic.cu — generic persistent window kernel (any topology of Input / McCullochPitts / IF / LIF / BoostedLIF /
-// CurrentLIF / DiehlAndCook populations joined by dense and convolutional connections).
+// CurrentLIF / DiehlAndCook populations joined by dense, convolutional and sparse connections).
 //
 // One cooperative grid iterates the whole T-step window of Network.run (reference:
 // bindsnet/network/network.py:380-465) with at most four grid barriers per step and no host involvement.
@@ -15,7 +15,11 @@
 //   phase 3  unit = (connection, 32-column tile, chunk of source rows): STDP + decay + clamp
 //            (learning.py / MCC_learning.py); dense MSTDP by source tiles; conv rules spread over the grid
 //   barrier  (+ masks + barrier when Network.run got masks)
+// With a SparseConnection (the <CTAS, true> instantiation): a window pre-pass builds the column-block tables of the
+// patterns, and every step starts with the sparse gather (unit = (connection, column block, sample chunk)) and a
+// barrier; in one-step mode the gather of a layer's sparse inputs precedes that layer's phase 1.
 // After the last step: theta, normalize() by tiles (network.py:464-465).
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 
@@ -31,9 +35,22 @@ __device__ __forceinline__ void item_of(const DevNet &N, int item, int &li, int 
     tile = item - N.layers[li].item0;
 }
 
+// sparse gather unit u -> (connection, column block, sample chunk)
+__device__ __forceinline__ void sparse_unit(const DevNet &N, int u, int &c, int &blk, int &chunk) {
+    c = 0;
+    #pragma unroll 1
+    for (int cc = 0; cc < N.n_conns; ++cc)
+        if (N.conns[cc].kind == SNN_CONN_SPARSE && u >= N.sp[cc].first) c = cc;
+    const int v = u - N.sp[c].first;
+    blk = v % N.sp[c].nb;
+    chunk = v / N.sp[c].nb;
+}
+
 // CTAS = CTAs per SM the variant is compiled for: 2 (128 registers) is what runs by default — the 3-CTA variant's
 // 80-register budget makes it spill; it stays selectable for experiments (SNN_B200_GVAR=3).
-template <int CTAS>
+// SPARSE: the plan holds a SparseConnection.  Plans without one run the instantiation without the sparse phases, whose
+// code (and register allocation) is exactly what it is without the feature.
+template <int CTAS, bool SPARSE>
 __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(const __grid_constant__ DevNet N) {
 #ifdef SNN_EMU
     float *smem = emu::tls_cta->dyn_smem;
@@ -80,6 +97,8 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                 }
             }
     }
+    for (int c = 0; SPARSE && c < N.n_conns; ++c)   // column-block tables of the SparseConnections (checks the patterns)
+        if (N.conns[c].kind == SNN_CONN_SPARSE) sparse_prepass(N, c, blockIdx.x * SNN_GEN_WARPS + warp, G * SNN_GEN_WARPS);
     if (!grid_barrier(N.bar, G, N.err, bgen)) return;
     GPROF(7)
 
@@ -89,7 +108,16 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
             // spikes its predecessors produced in THIS step — a grid barrier per layer
             for (int l = 0; l < N.n_layers; ++l) {
                 const DevLayer &D = N.layers[l];
-                for (int u = blockIdx.x; u < D.nw * nch; u += G) phase1(N, l, u / nch, u % nch, t, M);
+                if (SPARSE) {   // the sparse inputs of this layer, from the spikes its phase 1 would read
+                    bool any = false;
+                    for (int u = blockIdx.x; u < N.sp_units; u += G) {
+                        int c, blk, ch; sparse_unit(N, u, c, blk, ch);
+                        if (N.conns[c].tgt == l) phase_sparse(N, c, blk, ch, N.conns[c].src < l, t, M);
+                    }
+                    for (int c = 0; c < N.n_conns; ++c) any |= N.conns[c].kind == SNN_CONN_SPARSE && N.conns[c].tgt == l;
+                    if (any && !grid_barrier(N.bar, G, N.err, bgen)) return;
+                }
+                for (int u = blockIdx.x; u < D.nw * nch; u += G) phase1<SPARSE>(N, l, u / nch, u % nch, t, M);
                 if (D.L.kind == SNN_NODE_DC && D.L.one_spike) {
                     if (!grid_barrier(N.bar, G, N.err, bgen)) return;
                     for (int u = blockIdx.x; u < D.nw * nch; u += G) phase2(N, l, u / nch, u % nch, t);
@@ -97,9 +125,18 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                 if (l + 1 < N.n_layers && !grid_barrier(N.bar, G, N.err, bgen)) return;
             }
         } else {
+            if (SPARSE) {   // sparse inputs of step t: spikes of step t - 1, values after step t - 1's decay
+                for (int u = blockIdx.x; u < N.sp_units; u += G) {
+                    int c, blk, ch; sparse_unit(N, u, c, blk, ch);
+                    phase_sparse(N, c, blk, ch, false, t, M);
+                }
+                GPROF(1)
+                if (!grid_barrier(N.bar, G, N.err, bgen)) return;
+                GPROF(2)
+            }
             for (int u = blockIdx.x; u < N.total_items * nch; u += G) {
                 int li, tile; item_of(N, u / nch, li, tile);
-                phase1(N, li, tile, u % nch, t, M);
+                phase1<SPARSE>(N, li, tile, u % nch, t, M);
             }
         }
         GPROF(0)
@@ -132,8 +169,10 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                 }
             }
             GPROF(4)
-            for (int c = 0; c < N.n_conns; ++c)
+            for (int c = 0; c < N.n_conns; ++c) {
                 if (N.conns[c].kind == SNN_CONN_CONV2D && N.conns[c].rule != SNN_RULE_NONE) phase3_conv(N, c, blockIdx.x, G, t, M);
+                if (SPARSE && N.conns[c].kind == SNN_CONN_SPARSE) decay_sparse(N.conns[c], blockIdx.x, G);
+            }
             GPROF(5)
             // the units of the learning phase are not the units that gather from the weights in the next step
             if (!grid_barrier(N.bar, G, N.err, bgen)) return;
@@ -194,7 +233,7 @@ static int plan_units(DevNet &N, int cap) {
         const snn_conn_t &C = N.conns[c];
         N.p3_first[c] = p3;
         N.p3_rc[c] = 0;
-        if (!N.learning || C.rule == SNN_RULE_NONE || C.kind == SNN_CONN_CONV2D) continue;
+        if (!N.learning || C.rule == SNN_RULE_NONE || C.kind == SNN_CONN_CONV2D || C.kind == SNN_CONN_SPARSE) continue;
         const int nwS = N.layers[C.src].nw, nwT = N.layers[C.tgt].nw;
         if (SNN_RULE_IS_MSTDP(C.rule)) { N.p3_rc[c] = 1; p3 += nwS; continue; }
         int rc = ceil_div(cap, nwT);
@@ -205,8 +244,17 @@ static int plan_units(DevNet &N, int cap) {
         p3 += nwT * rc;
     }
     N.p3_total = p3;
+    // sparse gather: (column block, chunk of SNN_GEN_WARPS samples) per SparseConnection (the blocks come from layout_generic)
+    int spu = 0;
+    for (int c = 0; c < N.n_conns; ++c)
+        if (N.conns[c].kind == SNN_CONN_SPARSE) {
+            N.sp[c].first = spu;
+            spu += N.sp[c].nb * ceil_div(N.B, SNN_GEN_WARPS);
+        }
+    N.sp_units = spu;
     long long units = (long long)N.total_items * N.nch;
     if (p3 > units) units = p3;
+    if (spu > units) units = spu;
     bool conv_rule = false;
     for (int c = 0; c < N.n_conns; ++c)
         if (N.learning && N.conns[c].kind == SNN_CONN_CONV2D && N.conns[c].rule != SNN_RULE_NONE) conv_rule = true;
@@ -221,7 +269,8 @@ int snn_generic_launch(DevNet &N, cudaStream_t) {
     int sms = 3;
     if (const char *v = getenv("SNN_EMU_SMS")) sms = atoi(v) > 0 ? atoi(v) : 3;
     const int grid = plan_units(N, sms * 2);
-    emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2>(*(const DevNet *)a); }, &N);
+    if (N.sp_units) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, true>(*(const DevNet *)a); }, &N);
+    else emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false>(*(const DevNet *)a); }, &N);
     return 0;
 }
 #else
@@ -233,14 +282,15 @@ int snn_generic_launch(DevNet &N, cudaStream_t stream) {
     if (e != cudaSuccess) return (int)e;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const size_t smem = snn_generic_smem_bytes(N.B);
-    // two CTAs per SM unless SNN_B200_GVAR=3 asks for the spilling three-CTA experiment
+    // two CTAs per SM unless SNN_B200_GVAR=3 asks for the spilling three-CTA experiment (plans without a SparseConnection)
+    const bool sparse = std::any_of(N.conns, N.conns + N.n_conns, [](const snn_conn_t &C) { return C.kind == SNN_CONN_SPARSE; });
     bool three = false;
-    if (const char *v = getenv("SNN_B200_GVAR")) three = v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
-    const void *kern = three ? (const void *)snn_generic_window<3> : (const void *)snn_generic_window<2>;
+    if (const char *v = getenv("SNN_B200_GVAR")) three = !sparse && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
+    const void *kern = three ? (const void *)snn_generic_window<3, false>
+                             : sparse ? (const void *)snn_generic_window<2, true> : (const void *)snn_generic_window<2, false>;
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
-    e = three ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, snn_generic_window<3>, SNN_GEN_THREADS, smem)
-              : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, snn_generic_window<2>, SNN_GEN_THREADS, smem);
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, SNN_GEN_THREADS, smem);
     if (e != cudaSuccess) return (int)e;
     if (per_sm < 1) return (int)cudaErrorLaunchOutOfResources;
     if (per_sm > (three ? 3 : 2)) per_sm = three ? 3 : 2;
@@ -258,7 +308,8 @@ int snn_generic_launch(DevNet &N, cudaStream_t stream) {
         static long long host[8 * 4096];
         cudaStreamSynchronize(stream);
         cudaMemcpy(host, prof_buf, sizeof(long long) * 8 * grid, cudaMemcpyDeviceToHost);
-        static const char *names[8] = {"phase1", "barrierA", "phase2", "barrierB", "phase3", "phase3conv", "barrierC", "prologue"};
+        const char *names[8] = {"phase1", "barrierA", "phase2", "barrierB", "phase3", "phase3conv", "barrierC", "prologue"};
+        if (N.sp_units) { names[1] = "sparse/bA"; names[2] = "sp.bar/ph2"; }   // with a SparseConnection: + gather, + its barrier
         fprintf(stderr, "[snn_b200 gprof] grid=%d x %d threads, nch=%d cs=%d p3_units=%d T=%d B=%d  (cycles per timestep: min / mean / max over CTAs)\n",
                 grid, SNN_GEN_THREADS, N.nch, N.cs, N.p3_total, N.T, N.B);
         for (int k = 0; k < 8; ++k) {

@@ -26,6 +26,40 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS) conn_compute_kernel(snn_conn_
     }
 }
 
+// SparseConnection.compute (topology.py:2009-2017, :332-346) on the CSR pattern: out[b,j] = the stored w[i,j] of the
+// spiking i, i ascending, from +0, then the bias — the window's sparse gather without its workspace: each lane (column j)
+// finds its entry of a spiking row by binary search.  Positions are clamped to [0, nnz], so a malformed pattern cannot make
+// it read outside the arrays.
+__global__ void __launch_bounds__(SNN_GEN_THREADS) sparse_compute_kernel(snn_conn_t C, int ns, int nt, int B,
+                                                                          const uint8_t *__restrict__ s, float *__restrict__ out) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int j = blockIdx.x * SNN_TILE + lane;
+    const bool valid = j < nt;
+    for (int b = blockIdx.y * SNN_GEN_WARPS + warp; b < B; b += gridDim.y * SNN_GEN_WARPS) {
+        float p = 0.0f;
+        for (int i0 = 0; i0 < ns; i0 += 32) {
+            const bool sp = (i0 + lane < ns) && s[(size_t)b * ns + i0 + lane] != 0;
+            uint32_t word = __ballot_sync(0xffffffffu, sp);
+            while (word) {
+                const int i = i0 + __ffs(word) - 1;
+                word &= word - 1;
+                const int a = max(0, min(C.sp_rowptr[i], C.nnz)), e = max(a, min(C.sp_rowptr[i + 1], C.nnz));
+                int lo = a, hi = e;
+                while (lo < hi) {
+                    const int mid = (lo + hi) >> 1;
+                    if (C.sp_col[mid] < j) lo = mid + 1; else hi = mid;
+                }
+                if (valid && lo < e && C.sp_col[lo] == j) p = p + C.w[lo];
+            }
+        }
+        if (valid) out[(size_t)b * nt + j] = C.b ? p + C.b[j] : p;
+    }
+}
+
+__global__ void __launch_bounds__(256) scale_kernel(float *w, size_t n, float f) {
+    for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (size_t)gridDim.x * blockDim.x) w[k] = w[k] * f;
+}
+
 // Conv2dConnection.compute (topology.py:799-815): out[b, co, oy, ox] = sum of the filter taps whose (zero-padded)
 // input position spiked, in ascending (ci, ky, kx) order, then the bias — the window kernels' gather_conv on
 // byte spikes.  Thread = one target neuron of one sample.
@@ -130,7 +164,8 @@ extern "C" {
 
 int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, int32_t B, const uint8_t *s, float *out,
                           void *stream) {
-    if (!conn || !conn->w || !s || !out || n_src <= 0 || n_tgt <= 0 || B <= 0) return SNN_ERR_BAD_ARG;
+    if (!conn || (!conn->w && !(conn->kind == SNN_CONN_SPARSE && conn->nnz == 0)) || !s || !out || n_src <= 0 || n_tgt <= 0 || B <= 0)
+        return SNN_ERR_BAD_ARG;
     if (conn->kind == SNN_CONN_CONV2D) {
         if (!conn->b || conn->cin * conn->hin * conn->win != n_src || conn->cout * conn->hout * conn->wout != n_tgt) return SNN_ERR_BAD_ARG;
         const size_t total = (size_t)B * n_tgt;
@@ -140,6 +175,11 @@ int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, 
     }
     dim3 grid((n_tgt + SNN_TILE - 1) / SNN_TILE, (B + SNN_GEN_WARPS - 1) / SNN_GEN_WARPS);
     if (grid.y > 64) grid.y = 64;
+    if (conn->kind == SNN_CONN_SPARSE) {
+        if (conn->nnz < 0 || !conn->sp_rowptr || (conn->nnz > 0 && !conn->sp_col)) return SNN_ERR_BAD_ARG;
+        SNN_LAUNCH(sparse_compute_kernel, grid, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
+        return cuda_rc(cudaGetLastError());
+    }
     SNN_LAUNCH(conn_compute_kernel, grid, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
     return cuda_rc(cudaGetLastError());
 }
@@ -147,7 +187,16 @@ int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, 
 int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *workspace, size_t workspace_bytes, void *stream_) {
     if (!net || ci < 0 || ci >= net->n_conns || B <= 0 || !workspace) return SNN_ERR_BAD_ARG;
     const snn_conn_t &C = net->conns[ci];
-    if (C.src < 0 || C.src >= net->n_layers || C.tgt < 0 || C.tgt >= net->n_layers || !C.w) return SNN_ERR_BAD_ARG;
+    if (C.src < 0 || C.src >= net->n_layers || C.tgt < 0 || C.tgt >= net->n_layers) return SNN_ERR_BAD_ARG;
+    if (C.kind == SNN_CONN_SPARSE) {   // learning.NoOp: the stored values decay (learning.py:93-94); no other rule on a fixed pattern
+        if (C.rule != SNN_RULE_NONE && C.rule != SNN_RULE_NOOP) return SNN_ERR_UNSUPPORTED;
+        if (C.nnz < 0 || (C.nnz > 0 && !C.w)) return SNN_ERR_BAD_ARG;
+        if (C.rule == SNN_RULE_NONE || C.nnz == 0 || C.weight_decay == 0.0f || C.weight_decay == 1.0f) return SNN_OK;
+        const int blocks = (int)(((size_t)C.nnz + 1023) / 1024 < 1184 ? ((size_t)C.nnz + 1023) / 1024 : 1184);
+        SNN_LAUNCH(scale_kernel, blocks, 256, 0, (cudaStream_t)stream_, C.w, (size_t)C.nnz, C.weight_decay);
+        return cuda_rc(cudaGetLastError());
+    }
+    if (!C.w) return SNN_ERR_BAD_ARG;
     // the single-operator update is the dense [n_src, n_tgt] rule application; convolutional weights and the
     // reward-modulated rules (whose state lives in the window plan) are only updated inside run_window
     if (C.kind != SNN_CONN_DENSE && C.kind != SNN_CONN_MCC) return SNN_ERR_UNSUPPORTED;
@@ -180,7 +229,9 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
 }
 
 int snn_b200_conn_normalize(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, void *stream) {
-    if (!conn || !conn->w || n_src <= 0 || n_tgt <= 0) return SNN_ERR_BAD_ARG;
+    if (!conn || n_src <= 0 || n_tgt <= 0) return SNN_ERR_BAD_ARG;
+    if (conn->kind == SNN_CONN_SPARSE) return SNN_ERR_UNSUPPORTED;   // the reference's normalize fails on a sparse w too
+    if (!conn->w) return SNN_ERR_BAD_ARG;
     if (!conn->has_norm) return SNN_OK;
     if (conn->kind == SNN_CONN_CONV2D) {
         const int F = conn->cout * conn->cin;

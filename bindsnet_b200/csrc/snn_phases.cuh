@@ -147,6 +147,128 @@ __device__ __forceinline__ float gather(const snn_conn_t &C, const uint32_t *__r
     return p;
 }
 
+// ---------------------------------------------------------------------------------------
+// SparseConnection (SNN_CONN_SPARSE, topology.py:2009-2017).  Both functions run alone between grid barriers and are
+// kept out of line, so that the register allocation of the rest of the window kernel does not depend on them.
+//
+// Window pre-pass: the column-block offset table of connection `c` (DevSparse::off), one warp per source row, rows spread
+// over every warp of the grid.  The pattern is checked on the way: a row whose rowptr is out of [0, nnz] or not monotone,
+// or whose columns are out of range or not strictly ascending, raises SNN_ERR_BAD_ARG and is entered as an empty row, so
+// that the gather never reads outside the arrays.
+__device__ __noinline__ void sparse_prepass(const DevNet &N, int c, int gwarp, int nwarps) {
+    const snn_conn_t &C = N.conns[c];
+    const DevSparse &P = N.sp[c];
+    const int ns = N.layers[C.src].L.n, nt = N.layers[C.tgt].L.n, nb = P.nb, bw = P.bw;
+    const int lane = threadIdx.x & 31;
+    const int32_t *__restrict__ col = C.sp_col;
+    for (int i = gwarp; i < ns; i += nwarps) {
+        const int a = __ldg(C.sp_rowptr + i), e = __ldg(C.sp_rowptr + i + 1);
+        bool bad = a < 0 || e < a || e > C.nnz;
+        if (!bad)
+            for (int p = a + lane; p < e; p += 32) {
+                const int cj = __ldg(col + p);
+                bad |= cj < 0 || cj >= nt || (p > a && cj <= __ldg(col + p - 1));
+            }
+        int32_t *o = P.off + (size_t)i * (nb + 1);
+        if (__any_sync(0xffffffffu, bad)) {
+            for (int k = lane; k <= nb; k += 32) o[k] = 0;
+            if (lane == 0 && N.err) atomicOr(N.err, SNN_ERR_BAD_ARG);
+            continue;
+        }
+        // o[k] = first position of the row with column >= k * bw: every k is written by exactly one lane
+        for (int p = a + lane; p < e; p += 32) {
+            const int kb = __ldg(col + p) / bw, kp = p > a ? __ldg(col + p - 1) / bw : -1;
+            for (int k = kp + 1; k <= kb; ++k) o[k] = p;
+        }
+        const int kl = e > a ? __ldg(col + e - 1) / bw : -1;
+        for (int k = kl + 1 + lane; k <= nb; k += 32) o[k] = e;
+    }
+}
+
+// Sparse gather, unit = (connection, column block, chunk of SNN_GEN_WARPS samples); warp w takes sample chunk * 8 + w.
+// The block's sums live in the warp's slice of the accumulator region (bw <= 1024 floats).  The warp compacts the
+// sample's spiking sources into an ascending list (1024 at a time, as the dense gather does), fetches the block segments
+// of 32 listed rows at once (one row per lane), then walks the rows in ascending order, eight rows' first 32 entries in
+// flight together; the lanes of a row touch distinct columns and a __syncwarp separates consecutive rows, so every
+// column is summed in ascending i from +0 — the dense gather's sum without its zero terms.  `cur`: the source's spikes
+// of this step (one-step mode) instead of the previous one.
+#define SNN_SPARSE_ROWS 8
+__device__ __noinline__ void phase_sparse(const DevNet &N, int c, int blk, int chunk, bool cur, int t, const GenSmem &M) {
+    const snn_conn_t &C = N.conns[c];
+    const DevSparse &P = N.sp[c];
+    const DevLayer &S = N.layers[C.src];
+    const int B = N.B, nt = N.layers[C.tgt].L.n, nb = P.nb, bw = P.bw;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int b = chunk * SNN_GEN_WARPS + warp;
+    if (b >= B) return;
+    const int j0 = blk * bw, jn = min(bw, nt - j0);
+    float *acc = M.acc + warp * SNN_GATHER_BLOCK;
+    uint16_t *lst = (uint16_t *)M.xs + warp * SNN_GATHER_BLOCK;
+    for (int x = lane; x < bw; x += 32) acc[x] = 0.0f;
+    __syncwarp();
+    const int slot = cur ? (t & 1) : ((t + 1) & 1);
+    const bool any = !S.anyf || __ldcg(S.anyf + (size_t)(cur ? t % 3 : (t + 2) % 3) * B + b) != 0u;
+    const int32_t *__restrict__ col = C.sp_col;
+    const float *__restrict__ wv = C.w;
+    const int32_t *__restrict__ offb = P.off + blk;
+    const uint32_t *sb = S.bits + ((size_t)slot * B + b) * S.nw;
+    for (int w0 = 0; any && w0 < S.nw; w0 += 32) {
+        uint32_t mine = w0 + lane < S.nw ? __ldcg(sb + w0 + lane) : 0u;
+        if (!__any_sync(0xffffffffu, mine != 0u)) continue;
+        const int cnt = __popc(mine);
+        int pre = cnt;
+        #pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, pre, o);
+            if (lane >= o) pre += v;
+        }
+        const int total = __shfl_sync(0xffffffffu, pre, 31);
+        int q = pre - cnt;
+        while (mine) {
+            const int r = __ffs(mine) - 1;
+            mine &= mine - 1;
+            lst[q++] = (uint16_t)((lane << 5) | r);
+        }
+        __syncwarp();
+        const size_t base = (size_t)w0 * 32;
+        for (int e0 = 0; e0 < total; e0 += 32) {
+            const int nr = min(32, total - e0);
+            int p0 = 0, p1 = 0;   // segment of my row in this block
+            if (lane < nr) {
+                const int32_t *o = offb + (base + lst[e0 + lane]) * (size_t)(nb + 1);
+                p0 = __ldcg(o);
+                p1 = __ldcg(o + 1);
+            }
+            for (int r0 = 0; r0 < nr; r0 += SNN_SPARSE_ROWS) {
+                int a[SNN_SPARSE_ROWS], e[SNN_SPARSE_ROWS], cj[SNN_SPARSE_ROWS];
+                float v[SNN_SPARSE_ROWS];
+                #pragma unroll
+                for (int k = 0; k < SNN_SPARSE_ROWS; ++k) {
+                    a[k] = __shfl_sync(0xffffffffu, p0, (r0 + k) & 31);
+                    e[k] = __shfl_sync(0xffffffffu, p1, (r0 + k) & 31);
+                    if (r0 + k >= nr) e[k] = a[k];
+                    const bool ok = a[k] + lane < e[k];
+                    cj[k] = ok ? __ldg(col + a[k] + lane) : j0;
+                    v[k] = ok ? __ldcg(wv + a[k] + lane) : 0.0f;
+                }
+                #pragma unroll
+                for (int k = 0; k < SNN_SPARSE_ROWS; ++k) {
+                    if (a[k] + lane < e[k]) acc[cj[k] - j0] = acc[cj[k] - j0] + v[k];
+                    for (int p = a[k] + 32 + lane; p < e[k]; p += 32) {   // rows with more than 32 entries in the block
+                        const int jj = __ldg(col + p) - j0;
+                        acc[jj] = acc[jj] + __ldcg(wv + p);
+                    }
+                    __syncwarp();
+                }
+            }
+        }
+        __syncwarp();   // the list is rewritten by the next group of words
+    }
+    __syncwarp();
+    for (int x = lane; x < jn; x += 32) P.out[(size_t)b * nt + j0 + x] = acc[x];
+    __syncwarp();   // the accumulator belongs to the warp's next unit
+}
+
 // Conv2dConnection.compute (topology.py:799-815) for one target neuron j = (co, oy, ox) of one
 // sample: the sum of the filter taps whose (zero-padded) input position spiked, in ascending
 // (ci, ky, kx) order, then the bias.  STAGED: the sample's source bit row and the filter taps of the
@@ -245,6 +367,7 @@ __device__ __forceinline__ bool finalize_neuron(const DevNet &N, const DevLayer 
 // ---------------------------------------------------------------------------------------
 // phase 1.  Work unit = (layer, 32-neuron tile, chunk of N.cs samples): one warp lane per neuron, the CTA's
 // warps stride over the chunk's samples.
+template <bool SPARSE>
 __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, const GenSmem &M) {
     const DevLayer &D = N.layers[li];
     const snn_layer_t &L = D.L;
@@ -365,7 +488,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
         #pragma unroll
         for (int q = 0; q < 4; ++q) {
             fwn[q] = 0u; afn[q] = 1u;
-            if (q < ncl && b < b1 && N.conns[cl[q]].kind != SNN_CONN_CONV2D) {
+            if (q < ncl && b < b1 && N.conns[cl[q]].kind != SNN_CONN_CONV2D && !(SPARSE && N.conns[cl[q]].kind == SNN_CONN_SPARSE)) {
                 const snn_conn_t &C = N.conns[cl[q]];
                 const DevLayer &S = N.layers[C.src];
                 const int slot = (N.one_step && C.src < li) ? wr : rd;
@@ -417,6 +540,9 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
                 } else {
                     p = gather_conv<false, false>(C, gsb, nullptr, 0, j, valid, c == conv_c ? geo : conv_geo(C, j, valid));
                 }
+            } else if (SPARSE && C.kind == SNN_CONN_SPARSE) {   // gathered by phase_sparse ahead of this phase
+                p = valid ? __ldcg(N.sp[c].out + (size_t)b * n + j) : 0.0f;
+                if (C.b && valid) p = p + C.b[j];
             } else {
                 const uint32_t *sbr = S.bits + ((size_t)slot * B + b) * S.nw;
                 if (!prefetched) first = lane < S.nw ? __ldcg(sbr + lane) : 0u;
@@ -1217,6 +1343,14 @@ __device__ void phase3_conv(const DevNet &N, int ci_, int cta, int ncta, int t, 
         }
         if (staged || stage_pm) __syncthreads();
     }
+}
+
+// learning.NoOp on a SparseConnection: every stored value *= weight_decay (learning.py:93-94), no clamp; spread over the
+// grid (cta of ncta).
+__device__ __forceinline__ void decay_sparse(const snn_conn_t &C, int cta, int ncta) {
+    if (C.rule != SNN_RULE_NOOP || C.weight_decay == 0.0f || C.weight_decay == 1.0f) return;
+    for (size_t k = (size_t)cta * SNN_GEN_THREADS + threadIdx.x; k < (size_t)C.nnz; k += (size_t)ncta * SNN_GEN_THREADS)
+        C.w[k] = __ldcg(C.w + k) * C.weight_decay;
 }
 
 // Conv2dConnection.normalize (topology.py:824-837): every (out, in) filter scaled to sum `norm`

@@ -86,6 +86,11 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
     if rule and hasattr(rule0, "_prepare"):  # rules with state of their own (MSTDP): allocate for this batch size / device
         rule0._prepare(B, conn.w.device, rule_kwargs or {})
     conn._fill_desc(d, dt, rule)
+    if d.kind == _abi.SNN_CONN_SPARSE:
+        fill_sparse(d, conn)
+        b = getattr(conn, "b", None)
+        d.b = _ptr(b) if b is not None else None
+        return
     w = conn.w
     if w.dtype != torch.float32 or not w.is_contiguous():
         raise TypeError("connection weights must be contiguous float32")
@@ -106,6 +111,47 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
             "learning rule was built with reduction=torch.squeeze (source.batch_size == 1 at construction) "
             f"but the run uses batch size {B}; pass reduction=torch.sum like the reference requires"
         )
+
+
+def fill_sparse(d: "_abi.SnnConn", conn) -> None:
+    """The CSR view of a ``SparseConnection``'s ``torch.sparse_coo`` weights.  An uncoalesced ``w`` (what NoOp's decay
+    leaves in the reference, or what a user assigns) is coalesced in place.  The int32 ``rowptr`` / ``col`` arrays are
+    built on the tensor's device and cached for as long as ``w``'s index tensor is unchanged; the values pointer is
+    ``w``'s own values, so the kernel's decay shows in the user's tensor."""
+    w = conn.w
+    if not w.is_sparse or w.sparse_dim() != 2 or w.dense_dim() != 0:
+        raise TypeError("SparseConnection.w must be a 2-D torch.sparse_coo tensor")
+    if w.dtype != torch.float32:
+        raise TypeError(f"SparseConnection.w must be float32, got {w.dtype}")
+    n_src, n_tgt = conn.source.n, conn.target.n
+    if tuple(w.shape) != (n_src, n_tgt):
+        raise ValueError(f"weight shape {tuple(w.shape)} != ({n_src}, {n_tgt})")
+    if not w.is_coalesced():
+        with torch.no_grad():
+            conn.w.data = w.coalesce()
+        w = conn.w
+    idx = w._indices()
+    nnz = idx.shape[1]
+    if nnz >= 2**31:
+        raise NotImplementedError(f"SparseConnection with {nnz} stored entries: the CUDA core indexes them with int32 (< 2**31)")
+    key = (idx.data_ptr(), idx._version, tuple(w.shape), str(idx.device))
+    cached = getattr(conn, "_b200_csr", None)
+    if cached is None or cached[0] != key:
+        with torch.no_grad():
+            counts = torch.bincount(idx[0], minlength=n_src)
+            rowptr = torch.zeros(n_src + 1, dtype=torch.int32, device=idx.device)
+            rowptr[1:] = torch.cumsum(counts, 0).to(torch.int32)
+            col = idx[1].to(torch.int32).contiguous()
+        # the index tensor stays referenced by the cache, so its address cannot be reused by another pattern
+        cached = (key, rowptr, col, idx)
+        conn._b200_csr = cached
+    vals = w._values()
+    if not vals.is_contiguous():
+        raise ValueError("SparseConnection.w values must be contiguous (they are updated in place by the CUDA core)")
+    d.w = _ptr(vals) if nnz > 0 else None
+    d.sp_rowptr = _ptr(cached[1])
+    d.sp_col = _ptr(cached[2]) if nnz > 0 else None
+    d.nnz = int(nnz)
 
 
 def network_device(network) -> torch.device:

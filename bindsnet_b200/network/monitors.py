@@ -154,6 +154,8 @@ class NetworkMonitor(AbstractMonitor):
             for c in self.connections:
                 obj = self.network.connections[c]
                 if hasattr(obj, v) and not (v == "w" and hasattr(obj, "pipeline")):
+                    if v == "w" and obj.w.is_sparse:
+                        raise NotImplementedError(f"NetworkMonitor does not record the sparse w of {c} (SparseConnection)")
                     yield c, v, obj, False
 
     def get(self) -> Dict:

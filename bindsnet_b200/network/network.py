@@ -201,7 +201,7 @@ class Network(torch.nn.Module):
     def _stage_conn_masks(self, masks, dev: torch.device):
         """``masks={(source, target): bool tensor}`` (network.py:279-280,321): weights to clamp to zero after every
         step's update (AbstractConnection.update, topology.py:127-131)."""
-        from .topology import Connection
+        from .topology import Connection, SparseConnection
 
         out = {}
         for key, m in (masks or {}).items():
@@ -210,6 +210,8 @@ class Network(torch.nn.Module):
             if key not in self.connections:
                 continue                                  # network.py:449 looks masks up per connection: unknown keys are ignored
             conn = self.connections[key]
+            if isinstance(conn, SparseConnection):
+                raise NotImplementedError("Mask isn't supported for SparseConnection")   # topology.py:129-131
             if hasattr(conn, "pipeline"):
                 continue                                  # MulticompartmentConnection.update ignores the kwarg (topology.py:509-518)
             if not isinstance(conn, Connection):
@@ -356,7 +358,7 @@ class Network(torch.nn.Module):
         for layer in self.layers.values():
             if type(layer) not in builtin_nodes and (layer.kind is None or type(layer).forward is not N.Nodes.forward):
                 return True
-        builtin_conns = (Tp.Connection, Tp.MulticompartmentConnection, Tp.Conv2dConnection, Tp.LocalConnection)
+        builtin_conns = (Tp.Connection, Tp.MulticompartmentConnection, Tp.Conv2dConnection, Tp.LocalConnection, Tp.SparseConnection)
         for conn in self.connections.values():
             if type(conn) not in builtin_conns:
                 return True

@@ -395,6 +395,73 @@ class LocalConnection(Connection):
         d.norm_abs = 0   # w *= norm / w.sum(0)  (topology.py:1476-1479)
 
 
+class SparseConnection(Connection):
+    """Sparse synapses (reference: topology.py:2009-2017): a ``Connection`` whose ``w`` is a ``torch.sparse_coo``
+    ``Parameter``.  A dense ``w`` (or none: dense random, as ``Connection`` draws it) is converted with ``to_sparse()``;
+    a sparse ``w`` is taken as given, so a large network never needs its dense matrix.  Inside ``Network.run`` the
+    generic window kernel gathers the stored entries only (in ascending source order, bit-identical to a dense
+    ``Connection`` holding the same values), and ``learning.NoOp(weight_decay=...)`` decays the stored values in place.
+
+    The pattern is fixed.  Any other learning rule is refused at construction: the reference's rules add an entry
+    wherever ``s_pre (x) x_post`` is non-zero (learning.py:403-417), which turns the pattern dense, and fail outright with
+    finite ``wmin`` / ``wmax`` (learning.py:101-102).  ``norm`` is refused at construction too; the reference accepts it
+    and fails in ``normalize()`` at the end of the first run.  ``masks=`` for it raise, as in the reference
+    (topology.py:129-131)."""
+
+    def __init__(
+        self,
+        source: Nodes,
+        target: Nodes,
+        nu: Optional[Union[float, Sequence[float], Sequence[torch.Tensor]]] = None,
+        reduction: Optional[callable] = None,
+        weight_decay: float = 0.0,
+        w_dtype: torch.dtype = torch.float32,
+        **kwargs,
+    ) -> None:
+        from ..learning import NoOp
+
+        rule = kwargs.get("update_rule", None)
+        if rule is not None and rule is not NoOp:
+            raise NotImplementedError(
+                f"SparseConnection keeps a fixed synapse pattern: learning rule {getattr(rule, '__name__', rule)} is not "
+                "supported (the reference's rules grow the pattern into a dense one; only learning.NoOp, i.e. static or "
+                "decaying weights, is)"
+            )
+        if kwargs.get("norm", None) is not None:
+            raise NotImplementedError(
+                "SparseConnection does not support norm: the reference's normalize() fails on a sparse w "
+                "(it would raise at the end of the first run; this raises at construction)"
+            )
+        w = kwargs.get("w", None)
+        if isinstance(w, torch.Tensor) and w.is_sparse:
+            if w_dtype != torch.float32:
+                raise NotImplementedError("bindsnet_b200 computes in float32 only (SURVEY.md §8b)")
+            AbstractConnection.__init__(self, source, target, nu, reduction, weight_decay, **kwargs)
+            if w.sparse_dim() != 2 or w.dense_dim() != 0 or tuple(w.shape) != (source.n, target.n):
+                raise ValueError(f"sparse w must be a 2-D sparse_coo tensor of shape ({source.n}, {target.n})")
+            w = self.cast_dtype_if_needed(w, w_dtype)
+            if (self.wmin != -np.inf).any() or (self.wmax != np.inf).any():      # topology.py:314-317
+                w = torch.sparse_coo_tensor(w._indices(), torch.clamp(w._values(), self.wmin, self.wmax), w.shape,
+                                            is_coalesced=w.is_coalesced())
+            self.w = Parameter(w.detach(), requires_grad=False)
+            b = kwargs.get("b", None)
+            self.b = Parameter(torch.as_tensor(b, dtype=torch.float32), requires_grad=False) if b is not None else None
+        else:
+            super().__init__(source, target, nu, reduction, weight_decay, w_dtype, **kwargs)
+            self.w = Parameter(self.w.to_sparse(), requires_grad=False)          # topology.py:2017
+
+    def update(self, **kwargs) -> None:
+        """topology.py:112-139 with the reference's refusal of masks on a sparse w (:129-131)."""
+        if kwargs.get("mask", None) is not None:
+            raise NotImplementedError("Mask isn't supported for SparseConnection")
+        super().update(**kwargs)
+
+    def _fill_desc(self, d: "_abi.SnnConn", dt: float, rule: bool = True) -> None:
+        super()._fill_desc(d, dt, rule)
+        d.kind = _abi.SNN_CONN_SPARSE
+        d.norm_abs = 0
+
+
 def _unsupported(name: str, where: str):
     class _Unsupported:
         __doc__ = f"``{name}`` (reference: {where}) — not on the accelerated path (SURVEY.md §8f)."
@@ -418,4 +485,3 @@ LocalConnection1D = _unsupported("LocalConnection1D", "topology.py:1487-1620")
 LocalConnection2D = _unsupported("LocalConnection2D", "topology.py:1623-1767")
 LocalConnection3D = _unsupported("LocalConnection3D", "topology.py:1770-1917")
 MeanFieldConnection = _unsupported("MeanFieldConnection", "topology.py:1920-2006")
-SparseConnection = _unsupported("SparseConnection", "topology.py:2009-2017")

@@ -114,7 +114,7 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
             raise NotImplementedError(f"MCC learning rule {name}")
     else:
         # Connection (topology.py:265-399) + learning.LearningRule (learning.py:31-104)
-        if type(conn).__name__ not in ("Connection", "LocalConnection"):
+        if type(conn).__name__ not in ("Connection", "LocalConnection", "SparseConnection"):
             raise NotImplementedError(f"{type(conn).__name__} is outside the accelerated path")
         rule = conn.update_rule
         d.kind = _abi.SNN_CONN_DENSE
@@ -141,6 +141,11 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
         d.has_clamp = int(finite and name != "NoOp")                                      # learning.py:97-104
         if conn.b is not None:
             d.b = conn.b.data_ptr()
+        if w.is_sparse:
+            # SparseConnection (topology.py:2009-2017): the torch.sparse_coo w as CSR.  NoOp's decay leaves it
+            # uncoalesced (learning.py:93-94); it is coalesced in place, and the values are the tensor's own
+            _fill_sparse(d, conn, keep)
+            return
     if w.dtype != torch.float32 or not w.is_contiguous():
         raise TypeError("weights must be contiguous float32")
     d.w = w.data_ptr()
@@ -153,6 +158,28 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
                 d.structure, d.structure_val = _abi.SNN_W_DIAG, _f(diag[0])
             elif bool(((w == w[0, 1]) | eye).all() & (diag == 0).all()):
                 d.structure, d.structure_val = _abi.SNN_W_OFFDIAG, _f(w[0, 1])
+
+
+def _fill_sparse(d: "_abi.SnnConn", conn, keep: List[torch.Tensor]) -> None:
+    d.kind = _abi.SNN_CONN_SPARSE
+    if d.rule not in (_abi.SNN_RULE_NOOP, _abi.SNN_RULE_NONE):
+        raise NotImplementedError("SparseConnection with a learning rule other than NoOp (the pattern would grow)")
+    if not conn.w.is_coalesced():
+        with torch.no_grad():
+            conn.w.data = conn.w.data.coalesce()
+    w = conn.w
+    if w.dtype != torch.float32:
+        raise TypeError("weights must be float32")
+    idx, vals = w._indices(), w._values()
+    if idx.shape[1] >= 2**31:
+        raise NotImplementedError("more than 2**31 - 1 stored synapses")
+    rowptr = torch.zeros(int(conn.source.n) + 1, dtype=torch.int32, device=idx.device)
+    rowptr[1:] = torch.cumsum(torch.bincount(idx[0], minlength=int(conn.source.n)), 0).to(torch.int32)
+    col = idx[1].to(torch.int32).contiguous()
+    keep += [rowptr, col]
+    d.nnz = int(idx.shape[1])
+    d.sp_rowptr, d.sp_col = rowptr.data_ptr(), col.data_ptr() if d.nnz else None
+    d.w = vals.data_ptr() if d.nnz else None
 
 
 def build_net(network, inputs: Dict[str, torch.Tensor], T: int, B: int):

@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define SNN_ABI_VERSION 9
+#define SNN_ABI_VERSION 10
 #define SNN_MAX_LAYERS 8
 #define SNN_MAX_CONNS 12
 
@@ -57,6 +57,12 @@ extern "C" {
 #define SNN_CONN_CONV2D 2 /* Conv2dConnection: F.conv2d(s.float(), w, b, stride, padding, dilation)
                              topology.py:799-815; w is [Cout, Cin, kh, kw], b is [Cout]; the source layer's
                              neurons are indexed (ci, y, x), the target's (co, oy, ox), row-major */
+#define SNN_CONN_SPARSE 3 /* SparseConnection: a Connection whose w is a torch.sparse_coo tensor, s.float() @ w + b
+                             topology.py:2009-2017, :332-346.  w holds the nnz stored values in CSR order (sp_rowptr /
+                             sp_col); out[b,j] = sum over the spiking i with a stored (i,j), i ascending, from +0, then
+                             + b[j] — bit-identical to the dense gather over the same values.  Fixed pattern: rules
+                             SNN_RULE_NONE / SNN_RULE_NOOP only (decay of the stored values), no normalize, no mask,
+                             generic tier only */
 
 /* ---- learning rules ---- */
 #define SNN_RULE_NONE 0        /* MCC_learning.NoOp: update() does nothing    MCC_learning.py:120-146 */
@@ -194,6 +200,12 @@ typedef struct snn_conn {
        w += et_coef * e_trace  with et_coef = nu[0] * dt * reward evaluated by the host in fp32 (:2232-2238). */
     float *e_trace;
     float e_trace_decay, tc_e_trace, et_coef;
+    /* SNN_CONN_SPARSE: compressed sparse rows of the [n_src, n_tgt] pattern.  sp_rowptr [n_src + 1], monotone, in
+       [0, nnz]; sp_col [nnz], strictly ascending within a row, < n_tgt; w [nnz] the values in the same order, decayed
+       in place by SNN_RULE_NOOP.  A malformed pattern is reported as SNN_ERR_BAD_ARG (in *err_flag by the window). */
+    const int32_t *sp_rowptr;
+    const int32_t *sp_col;
+    int32_t nnz;
 } snn_conn_t;
 
 typedef struct snn_net {

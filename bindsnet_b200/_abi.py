@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 
-SNN_ABI_VERSION = 10
+SNN_ABI_VERSION = 11
 SNN_MAX_LAYERS = 8
 SNN_MAX_CONNS = 12
 
@@ -130,6 +130,12 @@ class SnnConn(C.Structure):
         ("sp_rowptr", C.c_void_p),
         ("sp_col", C.c_void_p),
         ("nnz", C.c_int32),
+        ("f_prob", C.c_void_p),
+        ("f_mask", C.c_void_p),
+        ("f_int", C.c_void_p),
+        ("draw_seed", C.c_uint32),
+        ("draw_step", C.c_uint32),
+        ("draw_conn", C.c_uint32),
     ]
 
 
@@ -179,3 +185,20 @@ def one_spike_hash(seed: int, t: int, layer: int, b: int, j: int) -> int:
 
 def one_spike_key(seed: int, t: int, layer: int, b: int, j: int) -> int:
     return ((one_spike_hash(seed, t, layer, b, j) | 0x80000000) << 32) | j
+
+
+def synapse_draw(seed: int, t: int, conn: int, i: int, j: int) -> int:
+    """Python restatement of ``snn_synapse_draw`` (include/snn_b200.h): the Probability feature's hash of synapse (i, j)
+    of connection ``conn`` at step ``t``."""
+    h = _fmix32((seed ^ 0x53594E41) & 0xFFFFFFFF)
+    h = _fmix32((h ^ (0x9E3779B9 * (t + 1))) & 0xFFFFFFFF)
+    h = _fmix32((h ^ (0x85EBCA6B * (conn + 1))) & 0xFFFFFFFF)
+    h = _fmix32((h ^ (0xC2B2AE35 * (i + 1))) & 0xFFFFFFFF)
+    return _fmix32((h ^ (0x27D4EB2F * (j + 1))) & 0xFFFFFFFF)
+
+
+def synapse_transmits(h: int, p: float) -> bool:
+    """``snn_synapse_transmits``: (h >> 8) * 2**-24 < p, compared in float32 (exact: both sides are float32 values)."""
+    import numpy as np
+
+    return bool(np.float32((h >> 8) * 2.0**-24) < np.float32(p))

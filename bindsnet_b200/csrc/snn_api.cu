@@ -69,6 +69,7 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
         if (SNN_RULE_IS_STDP(C.rule) && (!net->layers[C.src].traces || !net->layers[C.tgt].traces))
             return SNN_ERR_BAD_ARG;
         if (C.mask && (C.kind != SNN_CONN_DENSE || SNN_RULE_IS_MSTDP(C.rule))) return SNN_ERR_UNSUPPORTED;
+        if ((C.f_prob || C.f_mask || C.f_int) && C.kind != SNN_CONN_MCC) return SNN_ERR_BAD_ARG;
     }
     return SNN_OK;
 }
@@ -76,6 +77,15 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
 static bool has_sparse(const snn_net_t *net) {
     for (int c = 0; c < net->n_conns; ++c)
         if (net->conns[c].kind == SNN_CONN_SPARSE) return true;
+    return false;
+}
+
+// some MulticompartmentConnection carries Probability / Mask / Intensity features
+static bool has_feat(const snn_net_t *net) {
+    for (int c = 0; c < net->n_conns; ++c) {
+        const snn_conn_t &C = net->conns[c];
+        if (C.f_prob || C.f_mask || C.f_int) return true;
+    }
     return false;
 }
 
@@ -158,14 +168,16 @@ extern "C" {
 int snn_b200_abi_version(void) { return SNN_ABI_VERSION; }
 
 const char *snn_b200_build_info(void) {
-    return "libsnn_b200 sm_90a (generic window + fused DC2015 windows v1/v2), ABI " "10" ", built " __DATE__ " " __TIME__;
+    return "libsnn_b200 sm_90a (generic window + fused DC2015 windows v1/v2), ABI " "11" ", built " __DATE__ " " __TIME__;
 }
 
 int snn_b200_last_launch_count(void) { return g_last_launches; }
 
 int snn_b200_select_tier(const snn_net_t *net, const snn_run_opts_t *opts) {
     if (validate(net, opts) != SNN_OK) return 0;
-    if (has_sparse(net))   // the fused DiehlAndCook2015 kernels (and so the delta windows) have no sparse gather
+    if (has_sparse(net) && has_feat(net)) return 0;   // one extra instantiation of the generic kernel each, not both
+    // the fused DiehlAndCook2015 kernels (and so the delta windows) have neither the sparse nor the feature gather
+    if (has_sparse(net) || has_feat(net))
         return (opts->tier == 0 || opts->tier == 1) && !opts->delta_w && !opts->delta_theta ? 1 : 0;
     if (opts->delta_w || opts->delta_theta)   // delta windows exist in the barrier kernel only
         return (opts->tier == 0 || opts->tier == 2) && snn_fused_dc_supported(net, opts) ? 2 : 0;
@@ -182,7 +194,7 @@ int snn_b200_select_tier(const snn_net_t *net, const snn_run_opts_t *opts) {
 size_t snn_b200_workspace_bytes(const snn_net_t *net, const snn_run_opts_t *opts) {
     if (validate(net, opts) != SNN_OK) return 0;
     size_t g = layout_generic(net, opts, nullptr, nullptr);
-    if (has_sparse(net)) return g;
+    if (has_sparse(net) || has_feat(net)) return g;
     size_t f = snn_fused_dc_supported(net, opts) ? snn_fused_dc_workspace_bytes(net, opts) : 0;
     size_t f2 = snn_fused_dc2_supported(net, opts) ? snn_fused_dc2_workspace_bytes(net, opts) : 0;
     if (f2 > f) f = f2;
@@ -219,6 +231,7 @@ int snn_b200_run_window(const snn_net_t *net, const snn_run_opts_t *opts, void *
         N.conns[c] = net->conns[c];
         const snn_conn_t &C = net->conns[c];
         if (C.mask) N.any_mask = 1;
+        if (C.f_prob || C.f_mask || C.f_int) N.any_feat = 1;
     }
     if (cudaMemsetAsync(N.bar, 0, sizeof(unsigned int) * 96, stream) != cudaSuccess) return SNN_ERR_CUDA;
     const int e = snn_generic_launch(N, stream);

@@ -96,6 +96,7 @@ struct DevNet {
     DevMstdp mst[SNN_MAX_CONNS];
     int32_t sp_units;             // sparse gather units of a step (0: the plan has no SparseConnection)
     DevSparse sp[SNN_MAX_CONNS];
+    int32_t any_feat;             // some MCC connection carries Probability / Mask / Intensity features
 };
 
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p) {

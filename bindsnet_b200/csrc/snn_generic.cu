@@ -50,7 +50,9 @@ __device__ __forceinline__ void sparse_unit(const DevNet &N, int u, int &c, int 
 // 80-register budget makes it spill; it stays selectable for experiments (SNN_B200_GVAR=3).
 // SPARSE: the plan holds a SparseConnection.  Plans without one run the instantiation without the sparse phases, whose
 // code (and register allocation) is exactly what it is without the feature.
-template <int CTAS, bool SPARSE>
+// FEAT: the plan holds a MulticompartmentConnection with Probability / Mask / Intensity features (snn_b200.h); only the
+// dense gather of phase 1 differs.  The two are not combined in one plan.
+template <int CTAS, bool SPARSE, bool FEAT>
 __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(const __grid_constant__ DevNet N) {
 #ifdef SNN_EMU
     float *smem = emu::tls_cta->dyn_smem;
@@ -117,7 +119,7 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                     for (int c = 0; c < N.n_conns; ++c) any |= N.conns[c].kind == SNN_CONN_SPARSE && N.conns[c].tgt == l;
                     if (any && !grid_barrier(N.bar, G, N.err, bgen)) return;
                 }
-                for (int u = blockIdx.x; u < D.nw * nch; u += G) phase1<SPARSE>(N, l, u / nch, u % nch, t, M);
+                for (int u = blockIdx.x; u < D.nw * nch; u += G) phase1<SPARSE, FEAT>(N, l, u / nch, u % nch, t, M);
                 if (D.L.kind == SNN_NODE_DC && D.L.one_spike) {
                     if (!grid_barrier(N.bar, G, N.err, bgen)) return;
                     for (int u = blockIdx.x; u < D.nw * nch; u += G) phase2(N, l, u / nch, u % nch, t);
@@ -136,7 +138,7 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
             }
             for (int u = blockIdx.x; u < N.total_items * nch; u += G) {
                 int li, tile; item_of(N, u / nch, li, tile);
-                phase1<SPARSE>(N, li, tile, u % nch, t, M);
+                phase1<SPARSE, FEAT>(N, li, tile, u % nch, t, M);
             }
         }
         GPROF(0)
@@ -269,8 +271,9 @@ int snn_generic_launch(DevNet &N, cudaStream_t) {
     int sms = 3;
     if (const char *v = getenv("SNN_EMU_SMS")) sms = atoi(v) > 0 ? atoi(v) : 3;
     const int grid = plan_units(N, sms * 2);
-    if (N.sp_units) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, true>(*(const DevNet *)a); }, &N);
-    else emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false>(*(const DevNet *)a); }, &N);
+    if (N.sp_units) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, true, false>(*(const DevNet *)a); }, &N);
+    else if (N.any_feat) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, true>(*(const DevNet *)a); }, &N);
+    else emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false>(*(const DevNet *)a); }, &N);
     return 0;
 }
 #else
@@ -282,12 +285,14 @@ int snn_generic_launch(DevNet &N, cudaStream_t stream) {
     if (e != cudaSuccess) return (int)e;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const size_t smem = snn_generic_smem_bytes(N.B);
-    // two CTAs per SM unless SNN_B200_GVAR=3 asks for the spilling three-CTA experiment (plans without a SparseConnection)
+    // two CTAs per SM unless SNN_B200_GVAR=3 asks for the spilling three-CTA experiment (plans without a SparseConnection
+    // or MCC features)
     const bool sparse = std::any_of(N.conns, N.conns + N.n_conns, [](const snn_conn_t &C) { return C.kind == SNN_CONN_SPARSE; });
     bool three = false;
-    if (const char *v = getenv("SNN_B200_GVAR")) three = !sparse && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
-    const void *kern = three ? (const void *)snn_generic_window<3, false>
-                             : sparse ? (const void *)snn_generic_window<2, true> : (const void *)snn_generic_window<2, false>;
+    if (const char *v = getenv("SNN_B200_GVAR")) three = !sparse && !N.any_feat && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
+    const void *kern = three ? (const void *)snn_generic_window<3, false, false>
+                     : sparse ? (const void *)snn_generic_window<2, true, false>
+                     : N.any_feat ? (const void *)snn_generic_window<2, false, true> : (const void *)snn_generic_window<2, false, false>;
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, SNN_GEN_THREADS, smem);

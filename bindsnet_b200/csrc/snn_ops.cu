@@ -26,6 +26,35 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS) conn_compute_kernel(snn_conn_
     }
 }
 
+// MulticompartmentConnection.compute with Probability / Mask / Intensity features (topology.py:437-479,
+// topology_features.py:425-429, :507-508, :755-756): conn_compute_kernel's sum over the spiking i, each term fl(w * I)
+// kept only when its mask byte is set and its draw under (draw_seed, draw_step, draw_conn) transmits — the window
+// gather's terms in the same order.
+__global__ void __launch_bounds__(SNN_GEN_THREADS) mcc_feat_compute_kernel(snn_conn_t C, int ns, int nt, int B,
+                                                                            const uint8_t *__restrict__ s, float *__restrict__ out) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int j = blockIdx.x * SNN_TILE + lane;
+    const bool valid = j < nt;
+    for (int b = blockIdx.y * SNN_GEN_WARPS + warp; b < B; b += gridDim.y * SNN_GEN_WARPS) {
+        float p = 0.0f;
+        for (int i0 = 0; i0 < ns; i0 += 32) {
+            const bool sp = (i0 + lane < ns) && s[(size_t)b * ns + i0 + lane] != 0;
+            uint32_t word = __ballot_sync(0xffffffffu, sp);
+            while (word) {
+                const int i = i0 + __ffs(word) - 1;
+                word &= word - 1;
+                if (!valid) continue;
+                const size_t ij = (size_t)i * nt + j;
+                bool keep = !C.f_mask || C.f_mask[ij] != 0;
+                if (keep && C.f_prob)
+                    keep = snn_synapse_transmits(snn_synapse_draw(C.draw_seed, C.draw_step, C.draw_conn, (uint32_t)i, (uint32_t)j), C.f_prob[ij]);
+                if (keep) p = p + (C.f_int ? C.w[ij] * C.f_int[ij] : C.w[ij]);
+            }
+        }
+        if (valid) out[(size_t)b * nt + j] = C.b ? p + C.b[j] : p;
+    }
+}
+
 // SparseConnection.compute (topology.py:2009-2017, :332-346) on the CSR pattern: out[b,j] = the stored w[i,j] of the
 // spiking i, i ascending, from +0, then the bias — the window's sparse gather without its workspace: each lane (column j)
 // finds its entry of a spiking row by binary search.  Positions are clamped to [0, nnz], so a malformed pattern cannot make
@@ -166,6 +195,8 @@ int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, 
                           void *stream) {
     if (!conn || (!conn->w && !(conn->kind == SNN_CONN_SPARSE && conn->nnz == 0)) || !s || !out || n_src <= 0 || n_tgt <= 0 || B <= 0)
         return SNN_ERR_BAD_ARG;
+    const bool feat = conn->f_prob || conn->f_mask || conn->f_int;
+    if (feat && conn->kind != SNN_CONN_MCC) return SNN_ERR_BAD_ARG;
     if (conn->kind == SNN_CONN_CONV2D) {
         if (!conn->b || conn->cin * conn->hin * conn->win != n_src || conn->cout * conn->hout * conn->wout != n_tgt) return SNN_ERR_BAD_ARG;
         const size_t total = (size_t)B * n_tgt;
@@ -178,6 +209,10 @@ int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, 
     if (conn->kind == SNN_CONN_SPARSE) {
         if (conn->nnz < 0 || !conn->sp_rowptr || (conn->nnz > 0 && !conn->sp_col)) return SNN_ERR_BAD_ARG;
         SNN_LAUNCH(sparse_compute_kernel, grid, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
+        return cuda_rc(cudaGetLastError());
+    }
+    if (feat) {
+        SNN_LAUNCH(mcc_feat_compute_kernel, grid, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
         return cuda_rc(cudaGetLastError());
     }
     SNN_LAUNCH(conn_compute_kernel, grid, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);

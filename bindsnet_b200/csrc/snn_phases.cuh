@@ -93,8 +93,14 @@ __device__ __forceinline__ float ld_ext(const snn_layer_t &L, size_t idx, bool &
 // `first` = the lane's word of block 0 (sb[lane]), loaded by the caller ahead of time.  The words of up to eight
 // blocks (8192 source neurons) are fetched together, so a wide but sparse source layer (the 6400 inhibitory neurons of
 // BASELINE config 3: 7 blocks, almost always empty) costs one L2 round trip instead of one per block.
+// FEAT: the connection may carry the MCC features f_prob / f_mask / f_int (snn_b200.h).  A visited synapse then adds
+// fl(w * I) only when its mask byte is set and its draw under (seed, step, conn) transmits; the Probability and Mask
+// factors are exact 0 / 1 in the reference, so dropping those terms leaves the reference's sum.  With FEAT = false the
+// function is the plain gather.
+template <bool FEAT>
 __device__ __forceinline__ float gather(const snn_conn_t &C, const uint32_t *__restrict__ sb, int nw_src,
-                                        int n_src, int n_tgt, int j, bool valid, int lane, uint16_t *__restrict__ lst, uint32_t first) {
+                                        int n_src, int n_tgt, int j, bool valid, int lane, uint16_t *__restrict__ lst, uint32_t first,
+                                        uint32_t seed = 0u, uint32_t step = 0u, uint32_t conn = 0u) {
     float p = 0.0f;
     const float *__restrict__ wcol = C.w + j;
     for (int s0 = 0; s0 < nw_src; s0 += 256) {
@@ -136,6 +142,27 @@ __device__ __forceinline__ float gather(const snn_conn_t &C, const uint32_t *__r
                 for (int k = 0; k < 8; ++k) {
                     const int i = base + (int)lst[min(e + k, total - 1)];
                     v[k] = (valid && e + k < total && i < n_src) ? __ldcg(wcol + (size_t)i * n_tgt) : 0.0f;
+                }
+                if (FEAT) {
+                    float pr[8], in[8];
+                    uint8_t mk[8];
+                    #pragma unroll
+                    for (int k = 0; k < 8; ++k) {
+                        const int i = base + (int)lst[min(e + k, total - 1)];
+                        const bool ok = valid && e + k < total && i < n_src;
+                        const size_t ij = (size_t)i * n_tgt + j;
+                        pr[k] = (ok && C.f_prob) ? __ldcg(C.f_prob + ij) : 1.0f;
+                        mk[k] = (ok && C.f_mask) ? __ldcg(C.f_mask + ij) : (uint8_t)1;
+                        in[k] = (ok && C.f_int) ? __ldcg(C.f_int + ij) : 1.0f;
+                    }
+                    #pragma unroll
+                    for (int k = 0; k < 8; ++k) {
+                        const int i = base + (int)lst[min(e + k, total - 1)];
+                        bool keep = mk[k] != 0;
+                        if (C.f_prob) keep = keep && snn_synapse_transmits(snn_synapse_draw(seed, step, conn, (uint32_t)i, (uint32_t)j), pr[k]);
+                        if (C.f_int) v[k] = v[k] * in[k];
+                        if (!keep) v[k] = 0.0f;
+                    }
                 }
                 #pragma unroll
                 for (int k = 0; k < 8; ++k)
@@ -367,7 +394,7 @@ __device__ __forceinline__ bool finalize_neuron(const DevNet &N, const DevLayer 
 // ---------------------------------------------------------------------------------------
 // phase 1.  Work unit = (layer, 32-neuron tile, chunk of N.cs samples): one warp lane per neuron, the CTA's
 // warps stride over the chunk's samples.
-template <bool SPARSE>
+template <bool SPARSE, bool FEAT>
 __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, const GenSmem &M) {
     const DevLayer &D = N.layers[li];
     const snn_layer_t &L = D.L;
@@ -546,7 +573,8 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
             } else {
                 const uint32_t *sbr = S.bits + ((size_t)slot * B + b) * S.nw;
                 if (!prefetched) first = lane < S.nw ? __ldcg(sbr + lane) : 0u;
-                p = anysp ? gather(C, sbr, S.nw, S.L.n, n, j, valid, lane, lst, first) : 0.0f;
+                p = anysp ? gather<FEAT>(C, sbr, S.nw, S.L.n, n, j, valid, lane, lst, first, N.seed, (uint32_t)t + N.step_offset, (uint32_t)c)
+                          : 0.0f;
                 if (C.b && valid) p = p + C.b[j];
             }
             cur = cur + p;

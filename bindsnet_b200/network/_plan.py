@@ -102,9 +102,11 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
         d.structure, d.structure_val = weight_structure(conn, w)
     b = getattr(conn, "b", None)
     d.b = _ptr(b) if b is not None else None
+    if d.kind == _abi.SNN_CONN_MCC:
+        fill_features(d, conn)
     rule = getattr(conn, "update_rule", None)
     if rule is None and hasattr(conn, "pipeline"):
-        rule = conn.pipeline[0].learning_rule
+        rule = conn._weight().learning_rule
     if d.rule >= _abi.SNN_RULE_POSTPRE and getattr(rule, "_squeeze", False) and B != 1:
         # The reference would fail inside torch with a broadcast error (SURVEY.md §0.9).
         raise RuntimeError(
@@ -152,6 +154,51 @@ def fill_sparse(d: "_abi.SnnConn", conn) -> None:
     d.sp_rowptr = _ptr(cached[1])
     d.sp_col = _ptr(cached[2]) if nnz > 0 else None
     d.nnz = int(nnz)
+
+
+def _feature_matrix(f, conn, dtype: torch.dtype) -> torch.Tensor:
+    v = f.value
+    shape = (conn.source.n, conn.target.n)
+    if v.dtype != dtype or tuple(v.shape) != shape or not v.is_contiguous():
+        raise TypeError(f"{type(f).__name__} feature {f.name!r}: value must be a contiguous {dtype} tensor of shape {shape}, "
+                        f"got {v.dtype} {tuple(v.shape)}")
+    if v.device != conn.w.device:
+        raise ValueError(f"{type(f).__name__} feature {f.name!r} is on {v.device}, the Weight on {conn.w.device}")
+    return v
+
+
+def _mask_bytes(f, conn) -> Optional[torch.Tensor]:
+    """A Mask's value as [n_src, n_tgt] bytes, or None when it lets every spike pass.  A [n_src, n_tgt] bool value is
+    read in place; a scalar or broadcast one (topology_features.py:347-362) is expanded once and cached until the
+    value changes."""
+    v = f.value
+    shape = (conn.source.n, conn.target.n)
+    if tuple(v.shape) == shape and v.is_contiguous() and v.device == conn.w.device:
+        return _as_u8(v)
+    key = (v.data_ptr(), v._version, tuple(v.shape), str(v.device), str(conn.w.device))
+    cached = getattr(f, "_b200_bytes", None)
+    if cached is None or cached[0] != key:
+        with torch.no_grad():
+            full = torch.broadcast_to(v, shape)
+            u8 = None if bool(full.all()) else full.to(conn.w.device, torch.uint8).contiguous()
+        cached = (key, u8, v)
+        f._b200_bytes = cached
+    return cached[1]
+
+
+def fill_features(d: "_abi.SnnConn", conn) -> None:
+    """Probability / Mask / Intensity of a MulticompartmentConnection (snn_conn_t f_prob / f_mask / f_int)."""
+    feats = conn._features()
+    p, m, i = feats.get("Probability"), feats.get("Mask"), feats.get("Intensity")
+    d.f_prob = _ptr(_feature_matrix(p, conn, torch.float32)) if p is not None else None
+    d.f_mask = _ptr(_mask_bytes(m, conn)) if m is not None else None
+    d.f_int = _ptr(_feature_matrix(i, conn, torch.float32)) if i is not None else None
+
+
+def has_probability(conn) -> bool:
+    from .topology_features import Probability
+
+    return any(isinstance(f, Probability) for f in getattr(conn, "pipeline", ()))
 
 
 def network_device(network) -> torch.device:
@@ -228,14 +275,19 @@ def _conn_desc(conn, B: int, dt: float = 1.0, rule: bool = True) -> "_abi.SnnCon
     return d
 
 
-def compute_single_connection(conn, s: torch.Tensor) -> torch.Tensor:
-    """``conn.compute(s)``: ``[B, *target.shape]`` currents for spikes ``s``."""
+def compute_single_connection(conn, s: torch.Tensor, draw: Optional[Tuple[int, int, int]] = None) -> torch.Tensor:
+    """``conn.compute(s)``: ``[B, *target.shape]`` currents for spikes ``s``.  ``draw`` = (seed, step, connection index)
+    of a Probability feature's draw; by default a fresh seed from torch's CPU generator, step 0, index 0."""
     B = s.shape[0]
     _backend.require_cuda(conn.w, "connection weights")
     su8 = _as_u8(s if s.dtype in (torch.bool, torch.uint8) else (s != 0)).reshape(B, -1).contiguous()
     su8 = su8.to(conn.w.device)
     out = torch.empty(B, conn.target.n, dtype=torch.float32, device=conn.w.device)
     d = _conn_desc(conn, B, rule=False)
+    if d.f_prob:
+        if draw is None:
+            draw = (int(torch.randint(0, 2**31 - 1, (1,)).item()), 0, 0)
+        d.draw_seed, d.draw_step, d.draw_conn = draw[0] & 0xFFFFFFFF, draw[1] & 0xFFFFFFFF, draw[2]
     _backend.conn_compute(d, conn.source.n, conn.target.n, B, su8, out)
     return out.view(B, *conn.target.shape)
 

@@ -42,7 +42,8 @@ class Network(torch.nn.Module):
         self.train(learning)
         # network.py:114-117: the class is instantiated here; run() asks it for each window's reward
         self.reward_fn = reward_fn() if reward_fn is not None else None
-        #: seed of the last window's one_spike tie-break stream (see snn_one_spike_key)
+        #: seed of the last window's draws: the one_spike tie-break (snn_one_spike_key) and the Probability features'
+        #: synapse draws (snn_synapse_draw)
         self.last_one_spike_seed: Optional[int] = None
 
     # -- registry (network.py:119-161) ----------------------------------------------------
@@ -81,7 +82,8 @@ class Network(torch.nn.Module):
         ``inputs[l]`` has shape ``[time, batch, *layer.shape]`` (or the shorter forms the
         reference accepts, network.py:329-340).  Keyword arguments: ``clamp``, ``unclamp``,
         ``injects_v`` as in the reference (network.py:268-281).  Extensions: ``one_spike_seed``
-        fixes the tie-break stream of ``DiehlAndCookNodes(one_spike=True)``;
+        fixes the window's draws — the tie-break of ``DiehlAndCookNodes(one_spike=True)`` and the synapse draws of
+        ``Probability`` features (without it, a seed is drawn from torch's CPU generator);
         ``b200_normalize=False`` skips the end-of-run normalize (used by the multi-GPU combine,
         ``bindsnet_b200.distributed``).
         """
@@ -134,12 +136,18 @@ class Network(torch.nn.Module):
         current spikes: the sum of ``compute`` over those connections in insertion order (network.py:211-250).
         Inside a window the kernels do this themselves (the gather phase); this host form — one single-operator
         launch per connection — serves the scripted tier and callers that step a network by hand."""
+        from .topology import MulticompartmentConnection
+
         B = self.batch_size
         cur = {}
-        for (src, tgt), conn in self.connections.items():
+        draw = getattr(self, "_draw", None)   # (seed, step) of the scripted tier's current step
+        for k, ((src, tgt), conn) in enumerate(self.connections.items()):
             if layers is not None and tgt not in layers:
                 continue
-            out = conn.compute(self.layers[src].s)
+            if draw is not None and type(conn) is MulticompartmentConnection:
+                out = _plan.compute_single_connection(conn, self.layers[src].s, draw=(draw[0], draw[1], k))
+            else:
+                out = conn.compute(self.layers[src].s)
             out = out.view(B, *self.layers[tgt].shape).float()
             cur[tgt] = cur[tgt] + out if tgt in cur else out
         return cur
@@ -248,9 +256,11 @@ class Network(torch.nn.Module):
         unclamps = {k: self._stage_mask(k, v, T, dev, False) for k, v in (unclamp or {}).items() if v is not None}
         injects = {k: self._stage_mask(k, v, T, dev, True) for k, v in (injects_v or {}).items() if v is not None}
         if seed is None:
-            # only a one_spike population consumes the tie-break stream; a network without one leaves torch's generator
-            # alone (as the reference does: its only draw on the path is DiehlAndCookNodes' multinomial, nodes.py:1097-1105)
-            if any(getattr(l, "one_spike", False) for l in self.layers.values()):
+            # only a one_spike population and a Probability feature consume the window's draws; a network without either
+            # leaves torch's generator alone (as the reference does: its only draws on the path are DiehlAndCookNodes'
+            # multinomial, nodes.py:1097-1105, and Probability's bernoulli, topology_features.py:425-429)
+            if any(getattr(l, "one_spike", False) for l in self.layers.values()) or any(
+                    _plan.has_probability(c) for c in self.connections.values()):
                 seed = int(torch.randint(0, 2**31 - 1, (1,)).item())  # CPU generator: torch.manual_seed governs it
             else:
                 seed = 0
@@ -259,7 +269,7 @@ class Network(torch.nn.Module):
         if delta is not None and (self._scripted_required() or T <= 0):
             raise _backend.BackendError("b200_delta windows run on the fused DiehlAndCook2015 kernel only")
         if self._scripted_required():
-            return self._run_scripted(ext, T, normalize, clamps, unclamps, injects, self._conn_masks, bool(one_step))
+            return self._run_scripted(ext, T, normalize, clamps, unclamps, injects, self._conn_masks, bool(one_step), seed, step_offset)
 
         fused = {name: self._fusable_monitor(m) for name, m in self.monitors.items()}
         if any(layer is None for layer in fused.values()):
@@ -368,15 +378,23 @@ class Network(torch.nn.Module):
                 return True
         return False
 
-    def _run_scripted(self, ext, T, normalize, clamps, unclamps, injects, masks, one_step) -> None:
+    def _run_scripted(self, ext, T, normalize, clamps, unclamps, injects, masks, one_step, seed=0, step_offset=0) -> None:
         """Per-timestep executor with the reference's own control flow (network.py:380-465): inputs from the
         previous step's spikes in connection insertion order, layers in insertion order, clamp / unclamp /
-        injects_v, connection updates, monitors, end-of-run normalize."""
+        injects_v, connection updates, monitors, end-of-run normalize.  Probability features draw what the window
+        kernel draws for the same seed and step."""
+        try:
+            self._scripted_steps(ext, T, normalize, clamps, unclamps, injects, masks, one_step, seed, step_offset)
+        finally:
+            self._draw = None
+
+    def _scripted_steps(self, ext, T, normalize, clamps, unclamps, injects, masks, one_step, seed, step_offset) -> None:
         B = self.batch_size
         dev = self._device()
         get_inputs = self._get_inputs
 
         for t in range(T):
+            self._draw = (seed, step_offset + t)
             current = {} if one_step else get_inputs()
             for lname, layer in self.layers.items():                          # network.py:386-413
                 if one_step:

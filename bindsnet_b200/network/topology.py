@@ -260,9 +260,11 @@ class AbstractMulticompartmentConnection(ABC, Module):
 
 
 class MulticompartmentConnection(AbstractMulticompartmentConnection):
-    """Feature-pipeline connection (reference: topology.py:402-537).  The CUDA core executes
-    pipelines consisting of exactly one dense ``Weight`` feature — what every model in
-    ``bindsnet.models`` builds (models.py:185-236)."""
+    """Feature-pipeline connection (reference: topology.py:402-537).  The CUDA core executes pipelines of exactly one
+    dense ``Weight`` feature — what every model in ``bindsnet.models`` builds (models.py:185-236) — plus at most one
+    ``Probability``, ``Mask`` and ``Intensity`` feature each, in any order.  A spiking source then adds ``w * I`` to a
+    target where the mask holds and the synapse's draw transmits (topology.py:437-479); the order of the pipeline
+    does not change that single rounding."""
 
     def __init__(
         self,
@@ -280,21 +282,36 @@ class MulticompartmentConnection(AbstractMulticompartmentConnection):
         if self.traces:
             raise NotImplementedError("MulticompartmentConnection(traces=True) is not implemented by the CUDA core")
 
-    def _weight(self):
-        from .topology_features import Weight
+    def _features(self) -> dict:
+        """The pipeline by kind: exactly one Weight and at most one Probability, Mask and Intensity feature."""
+        from .topology_features import Intensity, Mask, Probability, Weight
 
-        if len(self.pipeline) != 1 or not isinstance(self.pipeline[0], Weight):
-            raise NotImplementedError(
-                "the CUDA core executes MulticompartmentConnection pipelines made of a single Weight feature"
-            )
-        return self.pipeline[0]
+        kinds = {}
+        for f in self.pipeline:
+            k = next((c for c in (Weight, Probability, Mask, Intensity) if isinstance(f, c)), None)
+            if k is None:
+                raise NotImplementedError(
+                    "the CUDA core executes MulticompartmentConnection pipelines of one Weight feature and at most one "
+                    f"Probability, Mask and Intensity feature each, not {type(f).__name__}"
+                )
+            if k.__name__ in kinds:
+                raise NotImplementedError(f"a MulticompartmentConnection pipeline with two {k.__name__} features is not implemented by the CUDA core")
+            kinds[k.__name__] = f
+        if "Weight" not in kinds:
+            raise NotImplementedError("the CUDA core executes MulticompartmentConnection pipelines with exactly one Weight feature")
+        return kinds
+
+    def _weight(self):
+        return self._features()["Weight"]
 
     @property
     def w(self) -> torch.Tensor:
         return self._weight().value
 
     def compute(self, s: torch.Tensor) -> torch.Tensor:
-        """Reference: topology.py:437-479 + Weight.compute topology_features.py:633-645."""
+        """Reference: topology.py:437-479 + Weight.compute topology_features.py:633-645.  With a Probability feature
+        every call is a new step of its own: it draws a fresh seed from torch's CPU generator, as a window without
+        ``one_spike_seed`` does."""
         from . import _plan
 
         return _plan.compute_single_connection(self, s)

@@ -1,8 +1,9 @@
 """Connection features — host-side mirror of ``bindsnet/network/topology_features.py``.
 
-Only ``Weight`` (reference: topology_features.py:575-671, base class :15-362) is on the
-accelerated path: it is the single feature every ``bindsnet.models`` network puts in a
-``MulticompartmentConnection`` pipeline (models.py:185-236).
+On the accelerated path are ``Weight`` (reference: topology_features.py:575-671, base class :15-362), the single
+feature every ``bindsnet.models`` network puts in a ``MulticompartmentConnection`` pipeline (models.py:185-236), and
+the three multiplicative features a pipeline may add to it: ``Probability`` (stochastic synapses, :365-464), ``Mask``
+(:467-549) and ``Intensity`` (:724-769).  Learning and normalisation act on the ``Weight`` only.
 """
 from __future__ import annotations
 
@@ -18,6 +19,8 @@ from .. import _abi
 
 class AbstractFeature(ABC):
     """Reference: topology_features.py:15-362."""
+
+    _value_dtype = torch.float32   # the value dtype the CUDA core reads
 
     def __init__(
         self,
@@ -57,7 +60,7 @@ class AbstractFeature(ABC):
             raise NotImplementedError("sparse feature values are not implemented by the CUDA core")
         if parent_feature is not None:
             raise NotImplementedError("feature linking (parent_feature) is not implemented by the CUDA core")
-        if value_dtype != torch.float32:
+        if value_dtype != self._value_dtype:
             raise NotImplementedError("bindsnet_b200 computes in float32 only (SURVEY.md §8b)")
 
         self.name = name
@@ -192,22 +195,142 @@ class Weight(AbstractFeature):
             d.rule = _abi.SNN_RULE_NONE
 
 
+def _scalar_value(cls: str, value) -> None:
+    """A Python number as the value: the reference fails on it in ``cast_dtype_if_needed`` (topology_features.py:146-153)."""
+    if isinstance(value, (int, float)):
+        raise AttributeError(f"'{type(value).__name__}' object has no attribute 'dtype'")
+
+
+def _no_learning(cls: str, learning_rule, norm) -> None:
+    from ..learning.MCC_learning import NoOp
+
+    if learning_rule is not None and learning_rule is not NoOp:
+        raise NotImplementedError(f"a learning rule on a {cls} feature is not implemented by the CUDA core (only the Weight learns)")
+    if norm is not None:
+        raise NotImplementedError(f"norm on a {cls} feature is not implemented by the CUDA core (only the Weight is normalised)")
+
+
+class Probability(AbstractFeature):
+    """Stochastic synapses (reference: topology_features.py:365-464): each step, synapse (i, j) transmits with probability
+    ``value[i, j]``, one draw for the whole batch (``torch.bernoulli(value)`` broadcast over the samples, :425-429).  The
+    draw is the counter-based ``snn_synapse_draw`` of include/snn_b200.h, keyed by the window's seed
+    (``Network.run(one_spike_seed=...)``, ``Network.last_one_spike_seed``), the step and the connection's position."""
+
+    def __init__(
+        self,
+        name: str,
+        value: Union[torch.Tensor, float, int] = None,
+        value_dtype: torch.dtype = torch.float32,
+        range: Optional[Sequence[float]] = None,
+        norm: Optional[Union[torch.Tensor, float, int]] = None,
+        learning_rule=None,
+        nu: Optional[Union[list, tuple]] = None,
+        reduction: Optional[callable] = None,
+        decay: float = 0.0,
+        parent_feature=None,
+        sparse: Optional[bool] = False,
+        batch_size: int = 1,
+    ) -> None:
+        r = [0, 1] if range is None else range
+        super().__init__(
+            name=name, value=value, value_dtype=value_dtype, range=r, norm=norm, learning_rule=learning_rule, nu=nu,
+            reduction=reduction, decay=decay, parent_feature=parent_feature, sparse=sparse, batch_size=batch_size,
+        )
+        # topology_features.py:445-464
+        if isinstance(r[0], torch.Tensor):
+            assert (r[0] >= 0).all(), f"Invalid range for feature {name}: a min value is less than 0"
+        elif isinstance(r[0], (float, int)):
+            assert r[0] >= 0, f"Invalid range for feature {name}: the min value is less than 0"
+        else:
+            assert False, f"Invalid range for feature {name}: the min value must be of type torch.Tensor, float, or int"
+        _scalar_value("Probability", value)
+        _no_learning("Probability", learning_rule, norm)
+
+    def prime_feature(self, connection, device, **kwargs) -> None:
+        """topology_features.py:434-443."""
+        if self.value is None:
+            lo, hi = self.range
+            self.initialize_value = lambda: torch.clamp(torch.rand(connection.source.n, connection.target.n, device=device), lo, hi)
+        super().prime_feature(connection, device, **kwargs)
+
+
+class Mask(AbstractFeature):
+    """Boolean synapse mask (reference: topology_features.py:467-549): ``True`` lets a spike pass.  A scalar or
+    broadcastable value is expanded to the ``[source.n, target.n]`` matrix on the host; an all-``True`` one is dropped."""
+
+    _value_dtype = torch.bool
+
+    def __init__(self, name: str, value: Union[torch.Tensor, float, int] = None, sparse: Optional[bool] = False,
+                 batch_size: int = 1) -> None:
+        # topology_features.py:485-505
+        if isinstance(value, torch.Tensor):
+            assert value.dtype == torch.bool, f"Mask must be of type bool, not {value.dtype}"
+        elif value is not None:
+            if not isinstance(value, bool):
+                raise AttributeError(f"'{type(value).__name__}' object has no attribute 'dtype'")
+            value = torch.tensor(value)
+        super().__init__(name=name, value=value, value_dtype=torch.bool, sparse=sparse, batch_size=batch_size)
+
+    def prime_feature(self, connection, device, **kwargs) -> None:
+        """topology_features.py:513-549 (the learning rule is MCC_learning.NoOp: a Mask never changes)."""
+        from ..learning.MCC_learning import NoOp
+
+        if self.is_primed:
+            return
+        self.is_primed = True
+        if self.value is None:
+            self.value = (torch.rand(connection.source.n, connection.target.n) > 0.99).to(device=device)
+        self.value = Parameter(self.value.detach().clone(), requires_grad=False).to(device)
+        f = self.value
+        if f.dim() > 1:   # topology_features.py:347-361: a matrix must be [source.n, target.n]; fewer dims broadcast
+            assert tuple(f.shape) == (connection.source.n, connection.target.n), (
+                f"Feature {self.name} has an incorrect shape of {f.shape}. Should be of shape "
+                f"{(connection.source.n, connection.target.n)}"
+            )
+        self.learning_rule = NoOp(connection=connection)
+
+
+class Intensity(AbstractFeature):
+    """Per-synapse multiplicative factor (reference: topology_features.py:724-769), by default in [-1, 1].  With a
+    ``Weight`` the term a spike carries is the single rounding of ``w * value``."""
+
+    def __init__(
+        self,
+        name: str,
+        value: Union[torch.Tensor, float, int] = None,
+        value_dtype: torch.dtype = torch.float32,
+        range: Optional[Sequence[float]] = None,
+        sparse: Optional[bool] = False,
+        batch_size: int = 1,
+    ) -> None:
+        super().__init__(name=name, value=value, value_dtype=value_dtype, range=range, sparse=sparse, batch_size=batch_size)
+        _scalar_value("Intensity", value)
+
+    def prime_feature(self, connection, device, **kwargs) -> None:
+        """topology_features.py:758-769.  The reference keeps the int64 tensor its default draw makes; its values
+        (-1, 0, 1) are stored as float32 here."""
+        if self.value is None:
+            lo, hi = self.range
+            self.initialize_value = lambda: torch.clamp(
+                torch.sign(torch.randint(-1, +2, (connection.source.n, connection.target.n))), lo, hi
+            ).to(torch.float32)
+        super().prime_feature(connection, device, **kwargs)
+
+
 def _unsupported(name: str, where: str):
     class _Unsupported:
         __doc__ = f"``{name}`` (reference: {where}) — not on the accelerated path."
 
         def __init__(self, *args, **kwargs):
             raise NotImplementedError(
-                f"the {name} feature is outside the hot path bindsnet_b200 implements (Weight only)"
+                f"the {name} feature is outside the hot path bindsnet_b200 implements (Weight, Probability, Mask, "
+                "Intensity): it makes every synapse carry a signal, so the spike gather would turn dense"
             )
 
     _Unsupported.__name__ = name
     return _Unsupported
 
 
-Probability = _unsupported("Probability", "topology_features.py:365-464")
-Mask = _unsupported("Mask", "topology_features.py:467-549")
 MeanField = _unsupported("MeanField", "topology_features.py:552-572")
 Bias = _unsupported("Bias", "topology_features.py:674-721")
-Intensity = _unsupported("Intensity", "topology_features.py:724-769")
 Degradation = _unsupported("Degradation", "topology_features.py:772-813")

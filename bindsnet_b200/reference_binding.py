@@ -88,10 +88,27 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
     d.src, d.tgt = src, tgt
     d.weight_decay, d.dt_scale = 1.0, 1.0
     if hasattr(conn, "pipeline"):
-        # MulticompartmentConnection (topology.py:402-537) with one Weight feature (topology_features.py:575-671)
-        if len(conn.pipeline) != 1 or type(conn.pipeline[0]).__name__ != "Weight":
-            raise NotImplementedError("only MulticompartmentConnection pipelines of exactly one Weight feature")
-        feat = conn.pipeline[0]
+        # MulticompartmentConnection (topology.py:402-537) with one Weight feature (topology_features.py:575-671) and at most
+        # one Probability (:365-464), Mask (:467-549) and Intensity (:724-769) feature each, in any order
+        kinds = [type(f).__name__ for f in conn.pipeline]
+        if kinds.count("Weight") != 1 or any(k not in ("Weight", "Probability", "Mask", "Intensity") or kinds.count(k) > 1 for k in kinds):
+            raise NotImplementedError("only MulticompartmentConnection pipelines of one Weight feature and at most one Probability, "
+                                      "Mask and Intensity feature each")
+        by = {type(f).__name__: f for f in conn.pipeline}
+        feat = by["Weight"]
+        shape = (conn.source.n, conn.target.n)
+        if "Probability" in by:                               # the window's draw: snn_synapse_draw(opts.seed, step, c, i, j)
+            p = by["Probability"].value.detach().to(torch.float32).contiguous()
+            keep.append(p)
+            d.f_prob = p.data_ptr()
+        if "Mask" in by:
+            m = _u8(torch.broadcast_to(by["Mask"].value.detach(), shape)).contiguous()
+            keep.append(m)
+            d.f_mask = m.data_ptr()
+        if "Intensity" in by:                                 # an int64 value (the default draw, :761-767) is -1 / 0 / 1
+            i = torch.broadcast_to(by["Intensity"].value.detach().to(torch.float32), shape).contiguous()
+            keep.append(i)
+            d.f_int = i.data_ptr()
         rule = feat.learning_rule                                                         # an MCC_learning instance after priming
         d.kind = _abi.SNN_CONN_MCC
         w = feat.value

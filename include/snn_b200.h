@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define SNN_ABI_VERSION 10
+#define SNN_ABI_VERSION 11
 #define SNN_MAX_LAYERS 8
 #define SNN_MAX_CONNS 12
 
@@ -206,6 +206,18 @@ typedef struct snn_conn {
     const int32_t *sp_rowptr;
     const int32_t *sp_col;
     int32_t nnz;
+    /* SNN_CONN_MCC with Probability / Mask / Intensity features besides its Weight (topology.py:437-479).  Each is an
+       [n_src, n_tgt] row-major matrix or NULL (feature absent).  A spiking source i adds fl(w[i,j] * f_int[i,j]) (just
+       w[i,j] without f_int) to target j when f_mask[i,j] != 0 and the Probability draw of synapse (i, j) transmits
+       (snn_synapse_transmits with f_prob[i,j]); otherwise it adds nothing.  The sum is the plain MCC gather's: i
+       ascending, from +0.  The draw is one [n_src, n_tgt] mask per step, shared by every sample of the batch
+       (torch.bernoulli(value) broadcast over B, topology_features.py:425-429).  The window draws with (opts.seed,
+       opts.step_offset + t, connection index); snn_b200_conn_compute with (draw_seed, draw_step, draw_conn).  Generic
+       tier only, and not in a plan that also holds an SNN_CONN_SPARSE connection. */
+    const float *f_prob;    /* Probability.value, each in [0, 1]                    topology_features.py:365-464 */
+    const uint8_t *f_mask;  /* Mask.value, 0 / 1 bytes                              topology_features.py:467-549 */
+    const float *f_int;     /* Intensity.value                                      topology_features.py:724-769 */
+    uint32_t draw_seed, draw_step, draw_conn;
 } snn_conn_t;
 
 typedef struct snn_net {
@@ -264,6 +276,27 @@ static inline SNN_HD uint32_t snn_one_spike_hash(uint32_t seed, uint32_t t, uint
 static inline SNN_HD uint64_t snn_one_spike_key(uint32_t seed, uint32_t t, uint32_t layer, uint32_t b, uint32_t j) {
     return ((uint64_t)(snn_one_spike_hash(seed, t, layer, b, j) | 0x80000000u) << 32) | (uint64_t)j;
 }
+
+/*
+ * Probability feature draw.  The reference transmits synapse (i, j) with torch.bernoulli(value): one [n_src, n_tgt]
+ * draw per MulticompartmentConnection.compute call, i.e. per step, broadcast over the batch (topology_features.py:
+ * 425-429).  We draw it from a counter-based 32-bit hash of (seed, step, connection, i, j): the source row is hashed
+ * once (snn_synapse_row), each column then costs one mixing round (snn_synapse_col).  The leading tag 0x53594E41
+ * keeps this stream apart from snn_one_spike_hash even under the same seed.  The synapse transmits when
+ * (h >> 8) * 2^-24 < p, exact in fp32: p = 0 never transmits, p = 1 always does.  The oracle, the kernels and the
+ * golden generator (which patches the reference's Probability.compute with it) share this definition.
+ */
+static inline SNN_HD uint32_t snn_synapse_row(uint32_t seed, uint32_t t, uint32_t conn, uint32_t i) {
+    uint32_t h = snn_fmix32(seed ^ 0x53594E41u);
+    h = snn_fmix32(h ^ (0x9E3779B9u * (t + 1u)));
+    h = snn_fmix32(h ^ (0x85EBCA6Bu * (conn + 1u)));
+    return snn_fmix32(h ^ (0xC2B2AE35u * (i + 1u)));
+}
+static inline SNN_HD uint32_t snn_synapse_col(uint32_t row, uint32_t j) { return snn_fmix32(row ^ (0x27D4EB2Fu * (j + 1u))); }
+static inline SNN_HD uint32_t snn_synapse_draw(uint32_t seed, uint32_t t, uint32_t conn, uint32_t i, uint32_t j) {
+    return snn_synapse_col(snn_synapse_row(seed, t, conn, i), j);
+}
+static inline SNN_HD int snn_synapse_transmits(uint32_t h, float p) { return (float)(h >> 8) * 5.9604644775390625e-08f < p; }
 
 /* Row-chunking of the end-of-window column sum (normalize): rows are split into
  * SNN_NORM_CHUNKS contiguous chunks of ceil(n_src/SNN_NORM_CHUNKS) rows, each summed in

@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 
-SNN_ABI_VERSION = 11
+SNN_ABI_VERSION = 12
 SNN_MAX_LAYERS = 8
 SNN_MAX_CONNS = 12
 

@@ -56,14 +56,15 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
             if (C.rule == SNN_RULE_MCC_POSTPRE) return SNN_ERR_UNSUPPORTED;
             if (SNN_RULE_IS_STDP(C.rule) && (C.dh != 1 || C.dw != 1)) return SNN_ERR_UNSUPPORTED;   // im2col_indices ignores dilation
         }
-        if (C.rule == SNN_RULE_MSTDPET) {   // dense, batch size 1 (learning.py:2187-2249)
-            if (C.kind != SNN_CONN_DENSE || o->B != 1) return SNN_ERR_UNSUPPORTED;
+        // dense or MCC Weight, batch size 1 (learning.py:2187-2249, MCC_learning.py:652-733)
+        if (C.rule == SNN_RULE_MSTDPET) {
+            if ((C.kind != SNN_CONN_DENSE && C.kind != SNN_CONN_MCC) || o->B != 1) return SNN_ERR_UNSUPPORTED;
             if (!C.p_plus || !C.p_minus || !C.mst_spre || !C.mst_spost || !C.e_trace) return SNN_ERR_BAD_ARG;
         }
         if (C.rule == SNN_RULE_MSTDP) {
             if (!C.p_plus || !C.p_minus) return SNN_ERR_BAD_ARG;
             if (C.kind == SNN_CONN_CONV2D) { if (!C.elig || C.dh != 1 || C.dw != 1) return SNN_ERR_BAD_ARG; }
-            else if (C.kind == SNN_CONN_DENSE) { if (!C.mst_spre || !C.mst_spost) return SNN_ERR_BAD_ARG; }
+            else if (C.kind == SNN_CONN_DENSE || C.kind == SNN_CONN_MCC) { if (!C.mst_spre || !C.mst_spost) return SNN_ERR_BAD_ARG; }
             else return SNN_ERR_UNSUPPORTED;
         }
         if (SNN_RULE_IS_STDP(C.rule) && (!net->layers[C.src].traces || !net->layers[C.tgt].traces))
@@ -168,7 +169,7 @@ extern "C" {
 int snn_b200_abi_version(void) { return SNN_ABI_VERSION; }
 
 const char *snn_b200_build_info(void) {
-    return "libsnn_b200 sm_90a (generic window + fused DC2015 windows v1/v2), ABI " "11" ", built " __DATE__ " " __TIME__;
+    return "libsnn_b200 sm_90a (generic window + fused DC2015 windows v1/v2), ABI " "12" ", built " __DATE__ " " __TIME__;
 }
 
 int snn_b200_last_launch_count(void) { return g_last_launches; }

@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from .. import _abi
-from .MCC_learning import _reduction_code
+from .MCC_learning import _EligibilityTrace, _RewardModulated, _reduction_code
 
 
 class LearningRule(ABC):
@@ -151,7 +151,7 @@ class Hebbian(LearningRule):
         _check_connection(self, connection)
 
 
-class MSTDP(LearningRule):
+class MSTDP(_RewardModulated, LearningRule):
     """Reward-modulated STDP (reference: learning.py:1440-2121): dense ``Connection``
     (``_connection_update`` :1504-1574) and ``Conv2dConnection`` (``_conv2d_connection_update``
     :1942-2015).  Rule state lives here like in the reference: ``p_plus``, ``p_minus`` and — for the
@@ -182,55 +182,30 @@ class MSTDP(LearningRule):
 
     def _prepare(self, B: int, dev: torch.device, run_kwargs: dict) -> None:
         """Allocate / validate the rule state for a window (learning.py:1519-1535, 1958-1961, 1979-1991)."""
-        if run_kwargs.get("reward", None) is None:
-            raise KeyError("reward")  # learning.py:1541: kwargs["reward"]
-        for key in ("reward", "a_plus", "a_minus"):
-            v = run_kwargs.get(key, None)
-            if isinstance(v, dict) or (isinstance(v, torch.Tensor) and v.numel() != 1):
-                raise NotImplementedError(f"run(..., {key}=...) must be a scalar for the CUDA core")
-        self._run_kwargs = run_kwargs
+        self._take_run_kwargs(run_kwargs)
         src, tgt = self.source, self.target
-
-        def ensure(name, shape, dtype=torch.float32):
-            t = getattr(self, name, None)
-            if not isinstance(t, torch.Tensor) or tuple(t.shape) != tuple(shape) or t.device != dev or t.dtype != dtype:
-                setattr(self, name, torch.zeros(*shape, dtype=dtype, device=dev))
-
         if self._conv:
-            ensure("p_plus", (B, *src.shape))
-            ensure("p_minus", (B, tgt.shape[0], tgt.shape[1] * tgt.shape[2]))
-            ensure("_elig", (B, *self.connection.w.shape))
+            self._ensure("p_plus", (B, *src.shape), dev)
+            self._ensure("p_minus", (B, tgt.shape[0], tgt.shape[1] * tgt.shape[2]), dev)
+            self._ensure("_elig", (B, *self.connection.w.shape), dev)
         else:
-            ensure("p_plus", (B, src.n))
-            ensure("p_minus", (B, tgt.n))
-            ensure("_spre", (B, src.n), torch.uint8)
-            ensure("_spost", (B, tgt.n), torch.uint8)
+            self._prepare_traces((B, src.n), (B, tgt.n), dev)
 
     @property
     def eligibility(self) -> torch.Tensor:
         """``[B, *w.shape]`` eligibility that the next update will apply (learning.py:1568-1572, 2005-2010)."""
         if self._conv:
             return self._elig
-        return torch.bmm(self.p_plus.unsqueeze(2), self._spost.float().unsqueeze(1)) + torch.bmm(
-            self._spre.float().unsqueeze(2), self.p_minus.unsqueeze(1))
+        return _RewardModulated.eligibility.fget(self)
 
     def _fill_desc(self, d: "_abi.SnnConn") -> None:
         super()._fill_desc(d)
-        rk = self._run_kwargs
-        dt = float(self.connection.dt)
-        d.reward = float(rk["reward"])
-        d.a_plus = float(rk["a_plus"]) if rk.get("a_plus", None) is not None else 1.0
-        d.a_minus = float(rk["a_minus"]) if rk.get("a_minus", None) is not None else -1.0
-        d.p_plus_decay = float(torch.exp(-dt / self.tc_plus))    # learning.py:1565 (fp32 tensor arithmetic)
-        d.p_minus_decay = float(torch.exp(-dt / self.tc_minus))  # learning.py:1567
-        d.p_plus, d.p_minus = self.p_plus.data_ptr(), self.p_minus.data_ptr()
+        self._fill_reward(d, float(self.connection.dt))
         if self._conv:
             d.elig = self._elig.data_ptr()
-        else:
-            d.mst_spre, d.mst_spost = self._spre.data_ptr(), self._spost.data_ptr()
 
 
-class MSTDPET(MSTDP):
+class MSTDPET(_EligibilityTrace, MSTDP):
     """Reward-modulated STDP with an eligibility trace on a dense ``Connection`` (reference: learning.py:2124-2249;
     ``_connection_update`` :2187-2249).  Batch size 1 only: the reference flattens the spikes of the whole batch into its
     ``[n]`` traces (:2214-2215), which only has a meaning for one sample.  Rule state like the reference's: ``p_plus [n_src]``,
@@ -246,27 +221,12 @@ class MSTDPET(MSTDP):
         self.tc_e_trace = torch.tensor(kwargs.get("tc_e_trace", 25.0))
 
     def _prepare(self, B: int, dev: torch.device, run_kwargs: dict) -> None:
-        if B != 1:
-            raise NotImplementedError("MSTDPET is defined for batch size 1 only (learning.py:2214-2215 flattens the batch)")
+        self._prepare_trace(B, tuple(self.connection.w.shape), dev)
         super()._prepare(B, dev, run_kwargs)
-        t = getattr(self, "eligibility_trace", None)
-        shape = tuple(self.connection.w.shape)
-        if not isinstance(t, torch.Tensor) or tuple(t.shape) != shape or t.device != dev:
-            self.eligibility_trace = torch.zeros(*shape, device=dev)
-
-    @property
-    def eligibility(self) -> torch.Tensor:
-        """``[n_src, n_tgt]`` (learning.py:2245-2247)."""
-        return torch.outer(self.p_plus.view(-1), self._spost.float().view(-1)) + torch.outer(self._spre.float().view(-1), self.p_minus.view(-1))
 
     def _fill_desc(self, d: "_abi.SnnConn") -> None:
         super()._fill_desc(d)
-        dt = float(self.connection.dt)
-        d.e_trace = self.eligibility_trace.data_ptr()
-        d.e_trace_decay = float(torch.exp(-dt / self.tc_e_trace))          # learning.py:2229
-        d.tc_e_trace = float(self.tc_e_trace)
-        # update = nu[0] * dt * reward * eligibility_trace (learning.py:2232): the scalar product in fp32, left to right
-        d.et_coef = float(self.nu[0].float() * dt * float(self._run_kwargs["reward"]))
+        self._fill_trace(d, float(self.connection.dt))
 
 
 def _unsupported(name: str, where: str):

@@ -83,6 +83,8 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
     do not involve the learning rule, whose plan entry may need a run's keyword arguments)."""
     d.src, d.tgt = src_idx, tgt_idx
     rule0 = getattr(conn, "update_rule", None)
+    if rule0 is None and hasattr(conn, "pipeline") and not conn.manual_update:
+        rule0 = conn._weight().learning_rule   # MulticompartmentConnection.update never reaches it with manual_update
     if rule and hasattr(rule0, "_prepare"):  # rules with state of their own (MSTDP): allocate for this batch size / device
         rule0._prepare(B, conn.w.device, rule_kwargs or {})
     conn._fill_desc(d, dt, rule)

@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define SNN_ABI_VERSION 11
+#define SNN_ABI_VERSION 12
 #define SNN_MAX_LAYERS 8
 #define SNN_MAX_CONNS 12
 
@@ -71,7 +71,9 @@ extern "C" {
 #define SNN_RULE_WDEP_POSTPRE 3/* learning.WeightDependentPostPre             learning.py:626-653     */
 #define SNN_RULE_MCC_POSTPRE 4 /* MCC_learning.PostPre._connection_update     MCC_learning.py:224-302 */
 #define SNN_RULE_MSTDP 5       /* learning.MSTDP: reward-modulated STDP; _connection_update learning.py:1504-1574
-                                  on SNN_CONN_DENSE, _conv2d_connection_update :1942-2015 on SNN_CONN_CONV2D */
+                                  on SNN_CONN_DENSE, _conv2d_connection_update :1942-2015 on SNN_CONN_CONV2D;
+                                  MCC_learning.MSTDP._connection_update MCC_learning.py:468-548 on SNN_CONN_MCC (the
+                                  same arithmetic as on SNN_CONN_DENSE, with the same fields and pointers) */
 #define SNN_RULE_HEBBIAN 6     /* learning.Hebbian: both terms positive, nu applied after the batch reduction;
                                   _connection_update learning.py:1110-1136, _conv2d_connection_update :1348-1380 */
 /* On SNN_CONN_CONV2D the rules SNN_RULE_POSTPRE (learning.py:457-497), SNN_RULE_WDEP_POSTPRE (:920-975) and
@@ -79,7 +81,8 @@ extern "C" {
  * post[co,k] = reduce_b sum_l s_tgt[b,co,l] * x_src_col[b,k,l]  (dilation 1), nu applied after the reduction. */
 #define SNN_RULE_MSTDPET 7     /* learning.MSTDPET on a dense Connection (learning.py:2187-2249): reward-modulated STDP with an
                                   eligibility TRACE; batch size 1 only (the reference flattens the spikes of the whole batch into
-                                  its [n] traces) */
+                                  its [n] traces).  Also MCC_learning.MSTDPET (MCC_learning.py:652-733) on SNN_CONN_MCC, with the
+                                  same fields and pointers as on SNN_CONN_DENSE */
 #define SNN_RULE_IS_MSTDP(r) ((r) == SNN_RULE_MSTDP || (r) == SNN_RULE_MSTDPET)
 #define SNN_RULE_IS_STDP(r) (((r) >= SNN_RULE_POSTPRE && (r) <= SNN_RULE_MCC_POSTPRE) || (r) == SNN_RULE_HEBBIAN)
 
@@ -177,8 +180,8 @@ typedef struct snn_conn {
     const float *b;    /* [n_tgt] bias or NULL (topology.py:345); CONV2D: [Cout]            */
     /* SNN_CONN_CONV2D geometry (topology.py:738-760): source [cin,hin,win], target [cout,hout,wout] */
     int32_t cin, hin, win, cout, hout, wout, kh, kw, sh, sw, ph, pw, dh, dw;
-    /* SNN_RULE_MSTDP (learning.py:1440-1574, 1942-2015).  State of the rule, updated in place:
-         DENSE : p_plus [B,n_src], p_minus [B,n_tgt]; the eligibility [B,n_src,n_tgt] of the previous
+    /* SNN_RULE_MSTDP (learning.py:1440-1574, 1942-2015; MCC_learning.py:392-551).  State of the rule, updated in place:
+         DENSE, MCC: p_plus [B,n_src], p_minus [B,n_tgt]; the eligibility [B,n_src,n_tgt] of the previous
                  step is NOT materialised: it is p_plus (x) s_post + s_pre (x) p_minus of that step, so
                  the spikes the rule saw last are kept instead (mst_spre [B,n_src], mst_spost [B,n_tgt],
                  one byte per neuron);
@@ -194,7 +197,7 @@ typedef struct snn_conn {
        forced to 0 after every step's update, learning or not (AbstractConnection.update, topology.py:127-131).  [n_src, n_tgt]
        bytes, SNN_CONN_DENSE only (MulticompartmentConnection.update ignores the kwarg, topology.py:509-518); NULL = none. */
     const uint8_t *mask;
-    /* SNN_RULE_MSTDPET (learning.py:2187-2249), dense, B = 1.  p_plus [n_src], p_minus [n_tgt], mst_spre / mst_spost as for
+    /* SNN_RULE_MSTDPET (learning.py:2187-2249; MCC_learning.py:554-738), SNN_CONN_DENSE or SNN_CONN_MCC, B = 1.  p_plus [n_src], p_minus [n_tgt], mst_spre / mst_spost as for
        SNN_RULE_MSTDP (the eligibility of the previous step is rebuilt from them); e_trace [n_src, n_tgt] is the rule's
        eligibility_trace, updated in place:  e_trace = e_trace * e_trace_decay + eligibility / tc_e_trace  (:2229-2230),
        w += et_coef * e_trace  with et_coef = nu[0] * dt * reward evaluated by the host in fp32 (:2232-2238). */

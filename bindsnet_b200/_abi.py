@@ -8,12 +8,12 @@ from __future__ import annotations
 
 import ctypes as C
 
-SNN_ABI_VERSION = 12
+SNN_ABI_VERSION = 13
 SNN_MAX_LAYERS = 8
 SNN_MAX_CONNS = 12
 
 SNN_NODE_INPUT, SNN_NODE_LIF, SNN_NODE_DC, SNN_NODE_IF, SNN_NODE_CURRENT_LIF, SNN_NODE_BOOSTED_LIF, SNN_NODE_MCP = 0, 1, 2, 3, 4, 5, 6
-SNN_CONN_DENSE, SNN_CONN_MCC, SNN_CONN_CONV2D, SNN_CONN_SPARSE = 0, 1, 2, 3
+SNN_CONN_DENSE, SNN_CONN_MCC, SNN_CONN_CONV2D, SNN_CONN_SPARSE, SNN_CONN_MAXPOOL2D = 0, 1, 2, 3, 4
 SNN_RULE_NONE, SNN_RULE_NOOP, SNN_RULE_POSTPRE, SNN_RULE_WDEP_POSTPRE, SNN_RULE_MCC_POSTPRE, SNN_RULE_MSTDP, SNN_RULE_HEBBIAN = 0, 1, 2, 3, 4, 5, 6
 SNN_RULE_MSTDPET = 7
 SNN_REDUCE_SUM, SNN_REDUCE_MEAN = 0, 1
@@ -136,6 +136,8 @@ class SnnConn(C.Structure):
         ("draw_seed", C.c_uint32),
         ("draw_step", C.c_uint32),
         ("draw_conn", C.c_uint32),
+        ("pool_rates", C.c_void_p),
+        ("pool_decay", C.c_float),
     ]
 
 

@@ -38,12 +38,17 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
     if ((o->delta_w || o->delta_theta) && (o->normalize || !net->learning || o->one_step)) return SNN_ERR_UNSUPPORTED;
     for (int c = 0; c < net->n_conns; ++c) {
         const snn_conn_t &C = net->conns[c];
-        const bool sparse = C.kind == SNN_CONN_SPARSE;
+        const bool sparse = C.kind == SNN_CONN_SPARSE, pool = C.kind == SNN_CONN_MAXPOOL2D;
         if (C.src < 0 || C.src >= net->n_layers || C.tgt < 0 || C.tgt >= net->n_layers) return SNN_ERR_BAD_ARG;
-        if (!C.w && !(sparse && C.nnz == 0)) return SNN_ERR_BAD_ARG;
+        if (pool ? (C.w || C.b) : (!C.w && !(sparse && C.nnz == 0))) return SNN_ERR_BAD_ARG;
         if (net->layers[C.tgt].kind == SNN_NODE_INPUT) return SNN_ERR_UNSUPPORTED;
         if (C.rule < SNN_RULE_NONE || C.rule > SNN_RULE_MSTDPET) return SNN_ERR_UNSUPPORTED;
-        if (C.kind < SNN_CONN_DENSE || C.kind > SNN_CONN_SPARSE) return SNN_ERR_UNSUPPORTED;
+        if (C.kind < SNN_CONN_DENSE || C.kind > SNN_CONN_MAXPOOL2D) return SNN_ERR_UNSUPPORTED;
+        if (pool) {   // no weights: learning.NoOp only, nothing to normalize or mask (snn_b200.h)
+            if (C.rule != SNN_RULE_NOOP || C.has_norm || C.mask) return SNN_ERR_UNSUPPORTED;
+            const int rc = snn_pool_geometry_ok(C, net->layers[C.src].n, net->layers[C.tgt].n);
+            if (rc != SNN_OK) return rc;
+        }
         if (sparse) {   // a fixed pattern: static or NoOp-decayed values, no normalize, no mask (snn_b200.h)
             if (C.rule != SNN_RULE_NONE && C.rule != SNN_RULE_NOOP) return SNN_ERR_UNSUPPORTED;
             if (C.has_norm || C.mask) return SNN_ERR_UNSUPPORTED;
@@ -73,6 +78,12 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
         if ((C.f_prob || C.f_mask || C.f_int) && C.kind != SNN_CONN_MCC) return SNN_ERR_BAD_ARG;
     }
     return SNN_OK;
+}
+
+static bool has_pool(const snn_net_t *net) {
+    for (int c = 0; c < net->n_conns; ++c)
+        if (net->conns[c].kind == SNN_CONN_MAXPOOL2D) return true;
+    return false;
 }
 
 static bool has_sparse(const snn_net_t *net) {
@@ -125,7 +136,8 @@ static size_t layout_generic(const snn_net_t *net, const snn_run_opts_t *o, char
         if (th) off += align_up(sizeof(int32_t) * 3 * L.n);
         bool wide_src = false;   // source of a dense connection with more than one gather block
         for (int c = 0; c < net->n_conns; ++c)
-            if (net->conns[c].src == l && net->conns[c].kind != SNN_CONN_CONV2D && nw > 32) wide_src = true;
+            if (net->conns[c].src == l && net->conns[c].kind != SNN_CONN_CONV2D && net->conns[c].kind != SNN_CONN_MAXPOOL2D && nw > 32)
+                wide_src = true;
         if (N) N->layers[l].anyf = wide_src ? (uint32_t *)(ws + off) : nullptr;
         if (wide_src) off += align_up(sizeof(uint32_t) * 3 * B);
         if (N && os) N->any_one_spike = 1;
@@ -161,6 +173,12 @@ static size_t layout_generic(const snn_net_t *net, const snn_run_opts_t *o, char
         if (N) N->sp[c].out = (float *)(ws + off);
         off += align_up(sizeof(float) * B * nt);
     }
+    // MaxPool2dConnections: the second slot of the rates (pool_rate_slot)
+    for (int c = 0; c < net->n_conns; ++c) {
+        if (net->conns[c].kind != SNN_CONN_MAXPOOL2D) continue;
+        if (N) N->pool_r1[c] = (float *)(ws + off);
+        off += align_up(sizeof(float) * B * (size_t)net->layers[net->conns[c].src].n);
+    }
     return off;
 }
 
@@ -169,16 +187,17 @@ extern "C" {
 int snn_b200_abi_version(void) { return SNN_ABI_VERSION; }
 
 const char *snn_b200_build_info(void) {
-    return "libsnn_b200 sm_90a (generic window + fused DC2015 windows v1/v2), ABI " "12" ", built " __DATE__ " " __TIME__;
+    return "libsnn_b200 sm_90a (generic window + fused DC2015 windows v1/v2), ABI " "13" ", built " __DATE__ " " __TIME__;
 }
 
 int snn_b200_last_launch_count(void) { return g_last_launches; }
 
 int snn_b200_select_tier(const snn_net_t *net, const snn_run_opts_t *opts) {
     if (validate(net, opts) != SNN_OK) return 0;
-    if (has_sparse(net) && has_feat(net)) return 0;   // one extra instantiation of the generic kernel each, not both
-    // the fused DiehlAndCook2015 kernels (and so the delta windows) have neither the sparse nor the feature gather
-    if (has_sparse(net) || has_feat(net))
+    // one extra instantiation of the generic kernel each for sparse, feature and pooling plans, not combinations
+    if ((int)has_sparse(net) + (int)has_feat(net) + (int)has_pool(net) > 1) return 0;
+    // the fused DiehlAndCook2015 kernels (and so the delta windows) have neither the sparse, the feature nor the pooling gather
+    if (has_sparse(net) || has_feat(net) || has_pool(net))
         return (opts->tier == 0 || opts->tier == 1) && !opts->delta_w && !opts->delta_theta ? 1 : 0;
     if (opts->delta_w || opts->delta_theta)   // delta windows exist in the barrier kernel only
         return (opts->tier == 0 || opts->tier == 2) && snn_fused_dc_supported(net, opts) ? 2 : 0;
@@ -195,7 +214,7 @@ int snn_b200_select_tier(const snn_net_t *net, const snn_run_opts_t *opts) {
 size_t snn_b200_workspace_bytes(const snn_net_t *net, const snn_run_opts_t *opts) {
     if (validate(net, opts) != SNN_OK) return 0;
     size_t g = layout_generic(net, opts, nullptr, nullptr);
-    if (has_sparse(net) || has_feat(net)) return g;
+    if (has_sparse(net) || has_feat(net) || has_pool(net)) return g;
     size_t f = snn_fused_dc_supported(net, opts) ? snn_fused_dc_workspace_bytes(net, opts) : 0;
     size_t f2 = snn_fused_dc2_supported(net, opts) ? snn_fused_dc2_workspace_bytes(net, opts) : 0;
     if (f2 > f) f = f2;
@@ -233,6 +252,7 @@ int snn_b200_run_window(const snn_net_t *net, const snn_run_opts_t *opts, void *
         const snn_conn_t &C = net->conns[c];
         if (C.mask) N.any_mask = 1;
         if (C.f_prob || C.f_mask || C.f_int) N.any_feat = 1;
+        if (C.kind == SNN_CONN_MAXPOOL2D) N.any_pool = 1;
     }
     if (cudaMemsetAsync(N.bar, 0, sizeof(unsigned int) * 96, stream) != cudaSuccess) return SNN_ERR_CUDA;
     const int e = snn_generic_launch(N, stream);

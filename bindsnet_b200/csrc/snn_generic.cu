@@ -52,7 +52,11 @@ __device__ __forceinline__ void sparse_unit(const DevNet &N, int u, int &c, int 
 // code (and register allocation) is exactly what it is without the feature.
 // FEAT: the plan holds a MulticompartmentConnection with Probability / Mask / Intensity features (snn_b200.h); only the
 // dense gather of phase 1 differs.  The two are not combined in one plan.
-template <int CTAS, bool SPARSE, bool FEAT>
+// POOL: the plan holds a MaxPool2dConnection: phase 1 gathers its pooled spikes, and every finalised spike of its source
+// advances its rates (pool_rate_step); the prologue writes the rates of step 0.  Not combined with SPARSE or FEAT.  The
+// barriers are those of the plain window: the rates a gather reads were written before the barrier that ends the previous
+// step (or, in one-step mode, before the barrier that ends the source layer).
+template <int CTAS, bool SPARSE, bool FEAT, bool POOL>
 __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(const __grid_constant__ DevNet N) {
 #ifdef SNN_EMU
     float *smem = emu::tls_cta->dyn_smem;
@@ -98,6 +102,19 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                     for (size_t k = start; k < ne; k += stride) Ms.el[1][k] = Ms.el[0][k];
                 }
             }
+        // MaxPool2dConnection rates of step 0: the caller's rates advanced by the incoming spikes s(-1); in one-step mode
+        // with the source earlier in the insertion order step 0 advances them itself, from slot pool_rate_slot(T, -1)
+        for (int c = 0; POOL && N.T > 0 && c < N.n_conns; ++c) {
+            const snn_conn_t &C = N.conns[c];
+            if (C.kind != SNN_CONN_MAXPOOL2D || C.src != li || j >= D.L.n) continue;
+            const bool cur = N.one_step && C.src < C.tgt;
+            float *dst = pool_rates_at(N, c, pool_rate_slot(N.T, cur ? -1 : 0));
+            for (int b = warp; b < N.B; b += SNN_GEN_WARPS) {
+                const size_t k = (size_t)b * D.L.n + j;
+                const float r = C.pool_rates[k];
+                dst[k] = cur ? r : pool_rate_update(r, C.pool_decay, D.L.s[k] != 0);
+            }
+        }
     }
     for (int c = 0; SPARSE && c < N.n_conns; ++c)   // column-block tables of the SparseConnections (checks the patterns)
         if (N.conns[c].kind == SNN_CONN_SPARSE) sparse_prepass(N, c, blockIdx.x * SNN_GEN_WARPS + warp, G * SNN_GEN_WARPS);
@@ -119,10 +136,10 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                     for (int c = 0; c < N.n_conns; ++c) any |= N.conns[c].kind == SNN_CONN_SPARSE && N.conns[c].tgt == l;
                     if (any && !grid_barrier(N.bar, G, N.err, bgen)) return;
                 }
-                for (int u = blockIdx.x; u < D.nw * nch; u += G) phase1<SPARSE, FEAT>(N, l, u / nch, u % nch, t, M);
+                for (int u = blockIdx.x; u < D.nw * nch; u += G) phase1<SPARSE, FEAT, POOL>(N, l, u / nch, u % nch, t, M);
                 if (D.L.kind == SNN_NODE_DC && D.L.one_spike) {
                     if (!grid_barrier(N.bar, G, N.err, bgen)) return;
-                    for (int u = blockIdx.x; u < D.nw * nch; u += G) phase2(N, l, u / nch, u % nch, t);
+                    for (int u = blockIdx.x; u < D.nw * nch; u += G) phase2<POOL>(N, l, u / nch, u % nch, t);
                 }
                 if (l + 1 < N.n_layers && !grid_barrier(N.bar, G, N.err, bgen)) return;
             }
@@ -138,7 +155,7 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
             }
             for (int u = blockIdx.x; u < N.total_items * nch; u += G) {
                 int li, tile; item_of(N, u / nch, li, tile);
-                phase1<SPARSE, FEAT>(N, li, tile, u % nch, t, M);
+                phase1<SPARSE, FEAT, POOL>(N, li, tile, u % nch, t, M);
             }
         }
         GPROF(0)
@@ -148,7 +165,7 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
             for (int u = blockIdx.x; u < N.total_items * nch; u += G) {
                 int li, tile; item_of(N, u / nch, li, tile);
                 const snn_layer_t &L = N.layers[li].L;
-                if (L.kind == SNN_NODE_DC && L.one_spike) phase2(N, li, tile, u % nch, t);
+                if (L.kind == SNN_NODE_DC && L.one_spike) phase2<POOL>(N, li, tile, u % nch, t);
             }
             GPROF(2)
         }
@@ -235,7 +252,8 @@ static int plan_units(DevNet &N, int cap) {
         const snn_conn_t &C = N.conns[c];
         N.p3_first[c] = p3;
         N.p3_rc[c] = 0;
-        if (!N.learning || C.rule == SNN_RULE_NONE || C.kind == SNN_CONN_CONV2D || C.kind == SNN_CONN_SPARSE) continue;
+        if (!N.learning || C.rule == SNN_RULE_NONE || C.kind == SNN_CONN_CONV2D || C.kind == SNN_CONN_SPARSE || C.kind == SNN_CONN_MAXPOOL2D)
+            continue;   // (a MaxPool2dConnection has no weights to update)
         const int nwS = N.layers[C.src].nw, nwT = N.layers[C.tgt].nw;
         if (SNN_RULE_IS_MSTDP(C.rule)) { N.p3_rc[c] = 1; p3 += nwS; continue; }
         int rc = ceil_div(cap, nwT);
@@ -271,9 +289,10 @@ int snn_generic_launch(DevNet &N, cudaStream_t) {
     int sms = 3;
     if (const char *v = getenv("SNN_EMU_SMS")) sms = atoi(v) > 0 ? atoi(v) : 3;
     const int grid = plan_units(N, sms * 2);
-    if (N.sp_units) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, true, false>(*(const DevNet *)a); }, &N);
-    else if (N.any_feat) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, true>(*(const DevNet *)a); }, &N);
-    else emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false>(*(const DevNet *)a); }, &N);
+    if (N.sp_units) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, true, false, false>(*(const DevNet *)a); }, &N);
+    else if (N.any_feat) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, true, false>(*(const DevNet *)a); }, &N);
+    else if (N.any_pool) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, true>(*(const DevNet *)a); }, &N);
+    else emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, false>(*(const DevNet *)a); }, &N);
     return 0;
 }
 #else
@@ -285,14 +304,15 @@ int snn_generic_launch(DevNet &N, cudaStream_t stream) {
     if (e != cudaSuccess) return (int)e;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const size_t smem = snn_generic_smem_bytes(N.B);
-    // two CTAs per SM unless SNN_B200_GVAR=3 asks for the spilling three-CTA experiment (plans without a SparseConnection
-    // or MCC features)
+    // two CTAs per SM unless SNN_B200_GVAR=3 asks for the spilling three-CTA experiment (plans without a SparseConnection,
+    // MCC features or a MaxPool2dConnection)
     const bool sparse = std::any_of(N.conns, N.conns + N.n_conns, [](const snn_conn_t &C) { return C.kind == SNN_CONN_SPARSE; });
     bool three = false;
-    if (const char *v = getenv("SNN_B200_GVAR")) three = !sparse && !N.any_feat && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
-    const void *kern = three ? (const void *)snn_generic_window<3, false, false>
-                     : sparse ? (const void *)snn_generic_window<2, true, false>
-                     : N.any_feat ? (const void *)snn_generic_window<2, false, true> : (const void *)snn_generic_window<2, false, false>;
+    if (const char *v = getenv("SNN_B200_GVAR")) three = !sparse && !N.any_feat && !N.any_pool && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
+    const void *kern = three ? (const void *)snn_generic_window<3, false, false, false>
+                     : sparse ? (const void *)snn_generic_window<2, true, false, false>
+                     : N.any_feat ? (const void *)snn_generic_window<2, false, true, false>
+                     : N.any_pool ? (const void *)snn_generic_window<2, false, false, true> : (const void *)snn_generic_window<2, false, false, false>;
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, SNN_GEN_THREADS, smem);

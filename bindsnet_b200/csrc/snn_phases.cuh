@@ -373,9 +373,55 @@ __device__ __forceinline__ float gather_conv(const snn_conn_t &C, const uint32_t
     return p + C.b[co];
 }
 
+// ---------------------------------------------------------------------------------------
+// MaxPool2dConnection (SNN_CONN_MAXPOOL2D, topology.py:1124-1211).
+//
+// The rates the gather of step t reads fold in the spikes that gather reads: step t - 1's (slot rd), or step t's in
+// one-step mode when the source comes earlier in the insertion order (`cur`).  Whoever finalises source neuron k of a
+// sample writes its next rate, one slot ahead of the readers: in step t the rates of step t + 1 (or, `cur`, of step t,
+// which its target reads after the layer barrier of one-step mode).  The window prologue writes the rates of step 0
+// from the caller's buffer and the incoming spikes.  No grid barrier is added.
+__device__ __forceinline__ void pool_rate_step(const DevNet &N, int li, size_t k, int t, bool sf) {
+    for (int c = 0; c < N.n_conns; ++c) {
+        const snn_conn_t &C = N.conns[c];
+        if (C.kind != SNN_CONN_MAXPOOL2D || C.src != li) continue;
+        const bool cur = N.one_step && C.src < C.tgt;
+        const int tw = cur ? t : t + 1;   // the step whose gather reads what is written here
+        if (tw >= N.T) continue;
+        const float r = __ldcg(pool_rates_at(N, c, pool_rate_slot(N.T, tw - 1)) + k);
+        pool_rates_at(N, c, pool_rate_slot(N.T, tw))[k] = pool_rate_update(r, C.pool_decay, sf);
+    }
+}
+
+// The source neuron whose spike target neuron j = (ch, oy, ox) of a sample receives: the first maximum of the rates `r`
+// ([C, hin, win] of that sample) over the window — row-major window order, padding never chosen, strict comparison (an
+// equal rate, -0 against +0 included, keeps the earlier element), a NaN taking over as it does in F.max_pool2d's CPU
+// kernel.  Plan validation (snn_pool_geometry_ok) guarantees a valid element in every window.
+__device__ __forceinline__ int pool_argmax(const snn_conn_t &C, const float *r, int j) {
+    const int L = C.hout * C.wout, ch = j / L, l = j - ch * L, oy = l / C.wout, ox = l - oy * C.wout;
+    const int HW = C.hin * C.win;
+    const float *rc = r + (size_t)ch * HW;
+    float best = 0.0f;
+    int idx = 0;
+    bool any = false;
+    for (int ky = 0; ky < C.kh; ++ky) {
+        const int iy = oy * C.sh - C.ph + ky * C.dh;
+        if (iy < 0 || iy >= C.hin) continue;
+        for (int kx = 0; kx < C.kw; ++kx) {
+            const int ix = ox * C.sw - C.pw + kx * C.dw;
+            if (ix < 0 || ix >= C.win) continue;
+            const float v = __ldcg(rc + iy * C.win + ix);
+            if (!any || v > best || v != v) { best = v; idx = iy * C.win + ix; any = true; }
+        }
+    }
+    return ch * HW + idx;
+}
+
 // Final spikes of one neuron of one sample: traces (nodes.py:96-103), clamp / unclamp (network.py:415-429),
-// recordings.  Returns the spike that is published.
-__device__ __forceinline__ bool finalize_neuron(const DevNet &N, const DevLayer &D, bool s, float xold, size_t k, int b, int j, int t, int wr) {
+// recordings, and (POOL) the next rate of every MaxPool2dConnection leaving the layer.  Returns the spike that is published.
+template <bool POOL>
+__device__ __forceinline__ bool finalize_neuron(const DevNet &N, const DevLayer &D, bool s, float xold, size_t k, int b, int j, int t, int wr,
+                                                int li) {
     const snn_layer_t &L = D.L;
     bool sf = s;
     if (L.traces) {
@@ -388,13 +434,14 @@ __device__ __forceinline__ bool finalize_neuron(const DevNet &N, const DevLayer 
     if (t == N.T - 1) L.s[k] = sf ? 1 : 0;
     if (L.rec_s) L.rec_s[((size_t)t * N.B + b) * L.n + j] = sf ? 1 : 0;
     if (L.rec_count && sf) L.rec_count[k] += 1;
+    if (POOL) pool_rate_step(N, li, k, t, sf);
     return sf;
 }
 
 // ---------------------------------------------------------------------------------------
 // phase 1.  Work unit = (layer, 32-neuron tile, chunk of N.cs samples): one warp lane per neuron, the CTA's
 // warps stride over the chunk's samples.
-template <bool SPARSE, bool FEAT>
+template <bool SPARSE, bool FEAT, bool POOL>
 __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, const GenSmem &M) {
     const DevLayer &D = N.layers[li];
     const snn_layer_t &L = D.L;
@@ -428,7 +475,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
                 bool sf = false;
                 if (valid) {
                     if (L.sum_input) L.summed[k] = L.summed[k] + (s ? 1.0f : 0.0f);
-                    sf = finalize_neuron(N, D, s, xo[q], k, b, j, t, wr);
+                    sf = finalize_neuron<POOL>(N, D, s, xo[q], k, b, j, t, wr, li);
                 }
                 const uint32_t fw = __ballot_sync(0xffffffffu, valid && sf);
                 if (lane == 0) {
@@ -515,7 +562,8 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
         #pragma unroll
         for (int q = 0; q < 4; ++q) {
             fwn[q] = 0u; afn[q] = 1u;
-            if (q < ncl && b < b1 && N.conns[cl[q]].kind != SNN_CONN_CONV2D && !(SPARSE && N.conns[cl[q]].kind == SNN_CONN_SPARSE)) {
+            if (q < ncl && b < b1 && N.conns[cl[q]].kind != SNN_CONN_CONV2D && !(SPARSE && N.conns[cl[q]].kind == SNN_CONN_SPARSE) &&
+                !(POOL && N.conns[cl[q]].kind == SNN_CONN_MAXPOOL2D)) {
                 const snn_conn_t &C = N.conns[cl[q]];
                 const DevLayer &S = N.layers[C.src];
                 const int slot = (N.one_step && C.src < li) ? wr : rd;
@@ -567,6 +615,11 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
                 } else {
                     p = gather_conv<false, false>(C, gsb, nullptr, 0, j, valid, c == conv_c ? geo : conv_geo(C, j, valid));
                 }
+            } else if (POOL && C.kind == SNN_CONN_MAXPOOL2D) {   // rates of this step: pool_rate_step / the prologue
+                const float *r = pool_rates_at(N, c, pool_rate_slot(N.T, t)) + (size_t)b * S.L.n;
+                const uint32_t *sb = S.bits + ((size_t)slot * B + b) * S.nw;
+                const int i = valid ? pool_argmax(C, r, j) : 0;
+                p = (valid && ((__ldcg(sb + (i >> 5)) >> (i & 31)) & 1u)) ? 1.0f : 0.0f;
             } else if (SPARSE && C.kind == SNN_CONN_SPARSE) {   // gathered by phase_sparse ahead of this phase
                 p = valid ? __ldcg(N.sp[c].out + (size_t)b * n + j) : 0.0f;
                 if (C.b && valid) p = p + C.b[j];
@@ -622,7 +675,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
             }
         } else {
             bool sf = false;
-            if (valid) sf = finalize_neuron(N, D, s, xold, k, b, j, t, wr);
+            if (valid) sf = finalize_neuron<POOL>(N, D, s, xold, k, b, j, t, wr, li);
             const uint32_t fw = __ballot_sync(0xffffffffu, valid && sf);
             if (lane == 0) {
                 D.bits[((size_t)wr * B + b) * nw + tile] = fw;
@@ -645,6 +698,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
 // ---------------------------------------------------------------------------------------
 // phase 2 (DiehlAndCookNodes with one_spike): keep the arg-max candidate of each sample
 // (nodes.py:1097-1105), then traces / clamp / publish as in phase 1.  Same work units as phase 1.
+template <bool POOL>
 __device__ void phase2(const DevNet &N, int li, int tile, int chunk, int t) {
     const DevLayer &D = N.layers[li];
     const snn_layer_t &L = D.L;
@@ -673,7 +727,7 @@ __device__ void phase2(const DevNet &N, int li, int tile, int chunk, int t) {
             const size_t k = (size_t)b * n + j;
             const bool s = valid && ((cand[q] >> lane) & 1u) && key[q] != 0ull && (uint32_t)(key[q] & 0xffffffffull) == (uint32_t)j;
             bool sf = false;
-            if (valid) sf = finalize_neuron(N, D, s, xo[q], k, b, j, t, wr);
+            if (valid) sf = finalize_neuron<POOL>(N, D, s, xo[q], k, b, j, t, wr, li);
             const uint32_t fw = __ballot_sync(0xffffffffu, valid && sf);
             if (lane == 0) {
                 D.bits[((size_t)wr * B + b) * nw + tile] = fw;

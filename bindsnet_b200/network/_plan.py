@@ -11,6 +11,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from .. import _abi, _backend
+from .topology import MaxPool2dConnection
 
 
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
@@ -87,6 +88,10 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
         rule0 = conn._weight().learning_rule   # MulticompartmentConnection.update never reaches it with manual_update
     if rule and hasattr(rule0, "_prepare"):  # rules with state of their own (MSTDP): allocate for this batch size / device
         rule0._prepare(B, conn.w.device, rule_kwargs or {})
+    if isinstance(conn, MaxPool2dConnection):   # no weights: the rates buffer and the geometry are all there is
+        conn._check((B, *conn.source.shape))
+        conn._fill_desc(d, dt, rule)
+        return
     conn._fill_desc(d, dt, rule)
     if d.kind == _abi.SNN_CONN_SPARSE:
         fill_sparse(d, conn)
@@ -261,11 +266,18 @@ def build_net(
                 d.rec_count = _ptr(r[2]); keep.append(r[2])
     masks = getattr(network, "_conn_masks", None) or {}
     for i, ((src, tgt), conn) in enumerate(network.connections.items()):
+        if network.learning and isinstance(conn, MaxPool2dConnection):
+            raise AttributeError(conn._no_w_message())   # the reference fails in the first step's update
         fill_conn(net.conns[i], conn, index[src], index[tgt], float(network.dt), B, network._rule_kwargs_of((src, tgt)))
         m = masks.get((src, tgt))
         if m is not None:
             net.conns[i].mask = _ptr(m)
             keep.append(m)
+    conns = [net.conns[i] for i in range(net.n_conns)]
+    if any(d.kind == _abi.SNN_CONN_MAXPOOL2D for d in conns) and any(
+            d.kind == _abi.SNN_CONN_SPARSE or d.f_prob or d.f_mask or d.f_int for d in conns):
+        raise NotImplementedError("a network with a MaxPool2dConnection and a SparseConnection or MulticompartmentConnection "
+                                  "features is not implemented by the CUDA core (each has its own instantiation of the window kernel)")
     return net, keep
 
 
@@ -281,6 +293,8 @@ def compute_single_connection(conn, s: torch.Tensor, draw: Optional[Tuple[int, i
     """``conn.compute(s)``: ``[B, *target.shape]`` currents for spikes ``s``.  ``draw`` = (seed, step, connection index)
     of a Probability feature's draw; by default a fresh seed from torch's CPU generator, step 0, index 0."""
     B = s.shape[0]
+    if isinstance(conn, MaxPool2dConnection):
+        return _compute_pool(conn, s)
     _backend.require_cuda(conn.w, "connection weights")
     su8 = _as_u8(s if s.dtype in (torch.bool, torch.uint8) else (s != 0)).reshape(B, -1).contiguous()
     su8 = su8.to(conn.w.device)
@@ -292,6 +306,21 @@ def compute_single_connection(conn, s: torch.Tensor, draw: Optional[Tuple[int, i
         d.draw_seed, d.draw_step, d.draw_conn = draw[0] & 0xFFFFFFFF, draw[1] & 0xFFFFFFFF, draw[2]
     _backend.conn_compute(d, conn.source.n, conn.target.n, B, su8, out)
     return out.view(B, *conn.target.shape)
+
+
+def _compute_pool(conn, s: torch.Tensor) -> torch.Tensor:
+    """``MaxPool2dConnection.compute(s)``: the rates advance in place, ``[B, C, Hout, Wout]`` pooled spikes."""
+    fr = conn.firing_rates
+    _backend.require_cuda(fr, "firing_rates")
+    conn._check(tuple(s.shape))
+    B = s.shape[0]
+    su8 = _as_u8(s if s.dtype in (torch.bool, torch.uint8) else (s != 0)).reshape(B, -1).contiguous().to(fr.device)
+    d = _abi.SnnConn()
+    conn._fill_desc(d, 1.0)
+    shape = (d.cout, d.hout, d.wout)
+    out = torch.empty(B, d.cout * d.hout * d.wout, dtype=torch.float32, device=fr.device)
+    _backend.conn_compute(d, conn.source.n, out.shape[1], B, su8, out)
+    return out.view(B, *shape)
 
 
 def _pair_net(conn, B: int) -> "_abi.SnnNet":

@@ -83,10 +83,35 @@ def fill_layer(d: "_abi.SnnLayer", layer, B: int, keep: List[torch.Tensor]) -> N
         d.one_spike = int(getattr(layer, "one_spike", False))
 
 
-def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep: Optional[List[torch.Tensor]] = None) -> None:
+def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep: Optional[List[torch.Tensor]] = None,
+                    B: Optional[int] = None, device: Optional[torch.device] = None) -> None:
+    """``B`` / ``device``: the run's batch size and the layers' device (default: the source layer's), against which a
+    MaxPool2dConnection's rates buffer is checked."""
     keep = keep if keep is not None else []
     d.src, d.tgt = src, tgt
     d.weight_decay, d.dt_scale = 1.0, 1.0
+    if type(conn).__name__ == "MaxPool2dConnection":
+        # topology.py:1124-1211: no weights; the firing_rates buffer is updated in place, so it must be [B, *source.shape]
+        # for this run (the window reads and writes B * n_src floats) and on the run's device.  The reference allocates it
+        # on the CPU at reset_state_variables (:1209-1211) and never resizes it when the batch size changes: move it to the
+        # layers' device and reset it after a batch change before binding a run.
+        from .network.topology import check_pool, pool_out_shape
+
+        B = int(conn.source.s.shape[0]) if B is None else int(B)
+        device = conn.source.s.device if device is None else torch.device(device)
+        check_pool(conn, (B, *conn.source.shape))   # the reference's RuntimeError / TypeError, raised before anything runs
+        fr = conn.firing_rates
+        if fr.device != device:
+            raise RuntimeError(f"MaxPool2dConnection.firing_rates is on {fr.device}, the run on {device}: move it to the "
+                               "layers' device first")
+        d.kind, d.rule = _abi.SNN_CONN_MAXPOOL2D, _abi.SNN_RULE_NOOP
+        d.cin, d.hin, d.win = (int(v) for v in conn.source.shape)
+        d.cout, d.hout, d.wout = pool_out_shape(conn)
+        (d.kh, d.kw), (d.sh, d.sw) = conn.kernel_size, conn.stride
+        (d.ph, d.pw), (d.dh, d.dw) = conn.padding, conn.dilation
+        d.pool_decay = _f(conn.decay)
+        d.pool_rates = fr.data_ptr()
+        return
     if hasattr(conn, "pipeline"):
         # MulticompartmentConnection (topology.py:402-537) with one Weight feature (topology_features.py:575-671) and at most
         # one Probability (:365-464), Mask (:467-549) and Intensity (:724-769) feature each, in any order
@@ -218,8 +243,13 @@ def build_net(network, inputs: Dict[str, torch.Tensor], T: int, B: int):
             net.layers[i].ext = x.data_ptr()
             net.layers[i].ext_dtype = _abi.SNN_EXT_F32 if x.dtype == torch.float32 else _abi.SNN_EXT_U8
             keep.append(x)
+    dev = next(iter(network.layers.values())).s.device
     for i, ((s, t), conn) in enumerate(network.connections.items()):
-        fill_connection(net.conns[i], conn, names.index(s), names.index(t), float(network.dt), keep)
+        if network.learning and type(conn).__name__ == "MaxPool2dConnection":
+            # the reference fails in the first step's update: learning.NoOp.update scales connection.w (learning.py:87-94)
+            raise AttributeError("'MaxPool2dConnection' object has no attribute 'w' (run MaxPool2dConnection networks with "
+                                 "learning off)")
+        fill_connection(net.conns[i], conn, names.index(s), names.index(t), float(network.dt), keep, B=B, device=dev)
     return net, keep
 
 

@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define SNN_ABI_VERSION 12
+#define SNN_ABI_VERSION 13
 #define SNN_MAX_LAYERS 8
 #define SNN_MAX_CONNS 12
 
@@ -63,6 +63,18 @@ extern "C" {
                              + b[j] — bit-identical to the dense gather over the same values.  Fixed pattern: rules
                              SNN_RULE_NONE / SNN_RULE_NOOP only (decay of the stored values), no normalize, no mask,
                              generic tier only */
+#define SNN_CONN_MAXPOOL2D 4 /* MaxPool2dConnection: online-rate max pooling, topology.py:1124-1211.  No weights (w, b NULL),
+                                rule SNN_RULE_NOOP only, no normalize, no mask.  Source [C,hin,win], target [C,hout,wout]
+                                (the conv geometry fields with cin = cout = C; kh/kw, sh/sw, ph/pw, dh/dw as for
+                                F.max_pool2d, no ceil mode).  Each compute:
+                                  1. r = fl(r - fl(pool_decay * r)); r = fl(r + s)   on pool_rates [B,C,hin,win], in place
+                                  2. idx = the first maximum of r[b,c] over the window, row-major window order, padding
+                                     never chosen (strict >, so -0 == +0 ties keep the earlier element)
+                                  3. out[b,c,oy,ox] = s[b,c,idx] as 0.0 / 1.0
+                                Inside a window the rates read by step t fold in the spikes that step's gather reads
+                                (step t - 1's, or step t's for an earlier layer in one-step mode), exactly as the
+                                reference's compute(source.s) does.  Generic tier only, and not in a plan that also holds
+                                an SNN_CONN_SPARSE connection or MCC features */
 
 /* ---- learning rules ---- */
 #define SNN_RULE_NONE 0        /* MCC_learning.NoOp: update() does nothing    MCC_learning.py:120-146 */
@@ -221,6 +233,11 @@ typedef struct snn_conn {
     const uint8_t *f_mask;  /* Mask.value, 0 / 1 bytes                              topology_features.py:467-549 */
     const float *f_int;     /* Intensity.value                                      topology_features.py:724-769 */
     uint32_t draw_seed, draw_step, draw_conn;
+    /* SNN_CONN_MAXPOOL2D (topology.py:1124-1211): the firing_rates buffer [B, C, hin, win], updated in place (after a
+       window it holds what the reference's buffer holds after the window's last compute), and the decay kwarg rounded
+       to fp32 as `decay * firing_rates` rounds it. */
+    float *pool_rates;
+    float pool_decay;
 } snn_conn_t;
 
 typedef struct snn_net {

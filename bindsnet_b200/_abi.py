@@ -13,6 +13,7 @@ SNN_MAX_LAYERS = 8
 SNN_MAX_CONNS = 12
 
 SNN_NODE_INPUT, SNN_NODE_LIF, SNN_NODE_DC, SNN_NODE_IF, SNN_NODE_CURRENT_LIF, SNN_NODE_BOOSTED_LIF, SNN_NODE_MCP = 0, 1, 2, 3, 4, 5, 6
+SNN_NODE_SUBIF, SNN_NODE_PASSTHROUGH = 7, 8
 SNN_CONN_DENSE, SNN_CONN_MCC, SNN_CONN_CONV2D, SNN_CONN_SPARSE, SNN_CONN_MAXPOOL2D = 0, 1, 2, 3, 4
 SNN_RULE_NONE, SNN_RULE_NOOP, SNN_RULE_POSTPRE, SNN_RULE_WDEP_POSTPRE, SNN_RULE_MCC_POSTPRE, SNN_RULE_MSTDP, SNN_RULE_HEBBIAN = 0, 1, 2, 3, 4, 5, 6
 SNN_RULE_MSTDPET = 7
@@ -34,7 +35,7 @@ ERR_NAMES = {
     SNN_ERR_UNSUPPORTED: "configuration not implemented by the CUDA core",
     SNN_ERR_WORKSPACE: "workspace too small",
     SNN_ERR_CUDA: "CUDA runtime error",
-    SNN_ERR_NONBINARY: "Input layer received values outside {0,1}",
+    SNN_ERR_NONBINARY: "Input layer received, or PassThroughNodes layer held or received, values outside {0,1}",
     SNN_ERR_BARRIER: "grid barrier timed out",
     SNN_ERR_STRUCTURE: "a static weight matrix no longer has the diagonal / constant off-diagonal structure it was planned with",
 }

@@ -26,10 +26,11 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
     if (o->T < 0 || o->B <= 0) return SNN_ERR_BAD_ARG;
     for (int l = 0; l < net->n_layers; ++l) {
         const snn_layer_t &L = net->layers[l];
-        if (L.kind < SNN_NODE_INPUT || L.kind > SNN_NODE_MCP) return SNN_ERR_UNSUPPORTED;
+        if (L.kind < SNN_NODE_INPUT || L.kind > SNN_NODE_PASSTHROUGH) return SNN_ERR_UNSUPPORTED;
         if (L.kind == SNN_NODE_CURRENT_LIF && !L.i) return SNN_ERR_BAD_ARG;
         if (L.n <= 0 || !L.s) return SNN_ERR_BAD_ARG;
-        if (L.kind != SNN_NODE_INPUT && (!L.v || (!L.refrac_count && L.kind != SNN_NODE_MCP))) return SNN_ERR_BAD_ARG;
+        const bool stateless = L.kind == SNN_NODE_INPUT || L.kind == SNN_NODE_PASSTHROUGH;
+        if (!stateless && (!L.v || (!L.refrac_count && L.kind != SNN_NODE_MCP))) return SNN_ERR_BAD_ARG;
         if (L.kind == SNN_NODE_DC && !L.theta) return SNN_ERR_BAD_ARG;
         if (L.traces && !L.x) return SNN_ERR_BAD_ARG;
         if (L.sum_input && !L.summed) return SNN_ERR_BAD_ARG;
@@ -76,13 +77,20 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
             return SNN_ERR_BAD_ARG;
         if (C.mask && (C.kind != SNN_CONN_DENSE || SNN_RULE_IS_MSTDP(C.rule))) return SNN_ERR_UNSUPPORTED;
         if ((C.f_prob || C.f_mask || C.f_int) && C.kind != SNN_CONN_MCC) return SNN_ERR_BAD_ARG;
+        // a PassThroughNodes layer carries 0 / 1 spikes: pooled ones in, none of a rule's traces (snn_b200.h)
+        const bool pass_src = net->layers[C.src].kind == SNN_NODE_PASSTHROUGH, pass_tgt = net->layers[C.tgt].kind == SNN_NODE_PASSTHROUGH;
+        if (pass_tgt && !pool) return SNN_ERR_UNSUPPORTED;
+        if ((pass_src || pass_tgt) && C.rule != SNN_RULE_NONE && C.rule != SNN_RULE_NOOP) return SNN_ERR_UNSUPPORTED;
     }
     return SNN_OK;
 }
 
+// the plan runs the pooling instantiation of the generic kernel: a MaxPool2dConnection, or a layer of ann_to_snn's kinds
 static bool has_pool(const snn_net_t *net) {
     for (int c = 0; c < net->n_conns; ++c)
         if (net->conns[c].kind == SNN_CONN_MAXPOOL2D) return true;
+    for (int l = 0; l < net->n_layers; ++l)
+        if (net->layers[l].kind == SNN_NODE_SUBIF || net->layers[l].kind == SNN_NODE_PASSTHROUGH) return true;
     return false;
 }
 
@@ -194,7 +202,8 @@ int snn_b200_last_launch_count(void) { return g_last_launches; }
 
 int snn_b200_select_tier(const snn_net_t *net, const snn_run_opts_t *opts) {
     if (validate(net, opts) != SNN_OK) return 0;
-    // one extra instantiation of the generic kernel each for sparse, feature and pooling plans, not combinations
+    // one extra instantiation of the generic kernel each for sparse, feature and pooling plans (pooling: also plans with
+    // SubtractiveResetIFNodes / PassThroughNodes), not combinations
     if ((int)has_sparse(net) + (int)has_feat(net) + (int)has_pool(net) > 1) return 0;
     // the fused DiehlAndCook2015 kernels (and so the delta windows) have neither the sparse, the feature nor the pooling gather
     if (has_sparse(net) || has_feat(net) || has_pool(net))
@@ -252,8 +261,8 @@ int snn_b200_run_window(const snn_net_t *net, const snn_run_opts_t *opts, void *
         const snn_conn_t &C = net->conns[c];
         if (C.mask) N.any_mask = 1;
         if (C.f_prob || C.f_mask || C.f_int) N.any_feat = 1;
-        if (C.kind == SNN_CONN_MAXPOOL2D) N.any_pool = 1;
     }
+    N.any_pool = has_pool(net) ? 1 : 0;
     if (cudaMemsetAsync(N.bar, 0, sizeof(unsigned int) * 96, stream) != cudaSuccess) return SNN_ERR_CUDA;
     const int e = snn_generic_launch(N, stream);
     if (e != 0) {

@@ -97,7 +97,8 @@ struct DevNet {
     int32_t sp_units;             // sparse gather units of a step (0: the plan has no SparseConnection)
     DevSparse sp[SNN_MAX_CONNS];
     int32_t any_feat;             // some MCC connection carries Probability / Mask / Intensity features
-    int32_t any_pool;             // some connection is a MaxPool2dConnection (SNN_CONN_MAXPOOL2D)
+    int32_t any_pool;             // some connection is a MaxPool2dConnection (SNN_CONN_MAXPOOL2D), or some layer is an
+                                  // SNN_NODE_SUBIF / SNN_NODE_PASSTHROUGH one: the plan runs the POOL instantiation
     float *pool_r1[SNN_MAX_CONNS];   // MaxPool2dConnection: the workspace slot of its rates (pool_rate_slot)
 };
 
@@ -239,6 +240,27 @@ __device__ __forceinline__ bool if_step(const snn_layer_t &L, float &v, float &r
     if (s) { rc = L.refrac; v = L.reset; }
     if (L.has_lbound && v < L.lbound) v = L.lbound;
     return s;
+}
+
+// SubtractiveResetIFNodes.forward (conversion/nodes.py:73-99): the gate is rc == 0 (a negative rc, left by
+// 0 < rc < dt, gates the next step's input off), the decrement keeps rc only while it is positive (else -0.0), and a
+// spike subtracts the threshold instead of resetting.
+__device__ __forceinline__ bool subif_step(const snn_layer_t &L, float &v, float &rc, float xin) {
+    const float gate = rc == 0.0f ? 1.0f : 0.0f;
+    v = v + gate * xin;
+    rc = (rc > 0.0f ? 1.0f : 0.0f) * (rc - L.dt);
+    const bool s = v >= L.thresh;
+    if (s) { rc = L.refrac; v = v - L.thresh; }
+    if (L.has_lbound && v < L.lbound) v = L.lbound;
+    return s;
+}
+
+// A PassThroughNodes layer's state s (float32 0.0 / 1.0, snn_b200.h) as a spike; any other value raises
+// SNN_ERR_NONBINARY.
+__device__ __forceinline__ bool passthrough_spike(const snn_layer_t &L, size_t k, int32_t *err) {
+    const float f = ((const float *)L.s)[k];
+    if (f != 0.0f && f != 1.0f && err) atomicOr(err, SNN_ERR_NONBINARY);
+    return f != 0.0f;
 }
 
 // CurrentLIFNodes.forward (nodes.py:770-791): decaying synaptic current `ic`, gate taken after the decrement.

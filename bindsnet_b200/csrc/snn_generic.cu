@@ -1,5 +1,6 @@
 // snn_generic.cu — generic persistent window kernel (any topology of Input / McCullochPitts / IF / LIF / BoostedLIF /
-// CurrentLIF / DiehlAndCook populations joined by dense, convolutional and sparse connections).
+// CurrentLIF / DiehlAndCook / SubtractiveResetIF / PassThrough populations joined by dense, convolutional, sparse and
+// pooling connections).
 //
 // One cooperative grid iterates the whole T-step window of Network.run (reference:
 // bindsnet/network/network.py:380-465) with at most four grid barriers per step and no host involvement.
@@ -52,7 +53,8 @@ __device__ __forceinline__ void sparse_unit(const DevNet &N, int u, int &c, int 
 // code (and register allocation) is exactly what it is without the feature.
 // FEAT: the plan holds a MulticompartmentConnection with Probability / Mask / Intensity features (snn_b200.h); only the
 // dense gather of phase 1 differs.  The two are not combined in one plan.
-// POOL: the plan holds a MaxPool2dConnection: phase 1 gathers its pooled spikes, and every finalised spike of its source
+// POOL: the plan holds a MaxPool2dConnection or a layer of ann_to_snn's kinds (SNN_NODE_SUBIF, SNN_NODE_PASSTHROUGH, whose
+// s is float32): phase 1 gathers the pooled spikes and steps those layers, and every finalised spike of a pooling source
 // advances its rates (pool_rate_step); the prologue writes the rates of step 0.  Not combined with SPARSE or FEAT.  The
 // barriers are those of the plain window: the rates a gather reads were written before the barrier that ends the previous
 // step (or, in one-step mode, before the barrier that ends the source layer).
@@ -77,7 +79,8 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
         const DevLayer &D = N.layers[li];
         const int j = tile * SNN_TILE + lane;
         for (int b = warp; b < N.B; b += SNN_GEN_WARPS) {
-            const bool s = j < D.L.n && D.L.s[(size_t)b * D.L.n + j] != 0;
+            const size_t k = (size_t)b * D.L.n + j;
+            const bool s = j < D.L.n && (POOL && D.L.kind == SNN_NODE_PASSTHROUGH ? passthrough_spike(D.L, k, N.err) : D.L.s[k] != 0);
             const uint32_t w = __ballot_sync(0xffffffffu, s);
             if (lane == 0) D.bits[((size_t)1 * N.B + b) * D.nw + tile] = w;
         }
@@ -112,7 +115,8 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
             for (int b = warp; b < N.B; b += SNN_GEN_WARPS) {
                 const size_t k = (size_t)b * D.L.n + j;
                 const float r = C.pool_rates[k];
-                dst[k] = cur ? r : pool_rate_update(r, C.pool_decay, D.L.s[k] != 0);
+                const bool sp = D.L.kind == SNN_NODE_PASSTHROUGH ? ((const float *)D.L.s)[k] != 0.0f : D.L.s[k] != 0;
+                dst[k] = cur ? r : pool_rate_update(r, C.pool_decay, sp);
             }
         }
     }

@@ -134,13 +134,14 @@ __global__ void __launch_bounds__(256) pool_compute_kernel(snn_conn_t C, int ns,
 
 __global__ void __launch_bounds__(SNN_GEN_THREADS) conv_normalize_kernel(snn_conn_t C) { normalize_conv_item(C, blockIdx.x, gridDim.x); }
 
-// bit-pack the CURRENT spikes of the two layers of a connection into slot 0
+// bit-pack the CURRENT spikes of the two layers of a connection into slot 0 (F32: a PassThroughNodes layer's float32 s)
+template <bool F32>
 __global__ void pack_bits_kernel(const uint8_t *__restrict__ s, uint32_t *__restrict__ bits, int B, int n, int nw) {
     const int lane = threadIdx.x & 31;
     const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (gw >= B * nw) return;
     const int b = gw / nw, w = gw % nw, j = w * 32 + lane;
-    const bool sp = j < n && s[(size_t)b * n + j] != 0;
+    const bool sp = j < n && (F32 ? ((const float *)s)[(size_t)b * n + j] != 0.0f : s[(size_t)b * n + j] != 0);
     const uint32_t word = __ballot_sync(0xffffffffu, sp);
     if (lane == 0) bits[(size_t)b * nw + w] = word;
 }
@@ -259,6 +260,8 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
         return cuda_rc(cudaGetLastError());
     }
     if (!C.w) return SNN_ERR_BAD_ARG;
+    const bool pass = net->layers[C.src].kind == SNN_NODE_PASSTHROUGH || net->layers[C.tgt].kind == SNN_NODE_PASSTHROUGH;
+    if (pass && C.rule != SNN_RULE_NONE && C.rule != SNN_RULE_NOOP) return SNN_ERR_UNSUPPORTED;   // (snn_b200.h)
     // the single-operator update is the dense [n_src, n_tgt] rule application; convolutional weights and the
     // reward-modulated rules (whose state lives in the window plan) are only updated inside run_window
     if (C.kind != SNN_CONN_DENSE && C.kind != SNN_CONN_MCC) return SNN_ERR_UNSUPPORTED;
@@ -282,7 +285,8 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
         D.xpub = D.L.x;  // slot 0 = the layer's current trace
         if (off > workspace_bytes) return SNN_ERR_WORKSPACE;
         const int warps = B * D.nw;
-        SNN_LAUNCH(pack_bits_kernel, (warps * 32 + 255) / 256, 256, 0, stream, D.L.s, D.bits, B, D.L.n, D.nw);
+        if (D.L.kind == SNN_NODE_PASSTHROUGH) SNN_LAUNCH(pack_bits_kernel<true>, (warps * 32 + 255) / 256, 256, 0, stream, D.L.s, D.bits, B, D.L.n, D.nw);
+        else SNN_LAUNCH(pack_bits_kernel<false>, (warps * 32 + 255) / 256, 256, 0, stream, D.L.s, D.bits, B, D.L.n, D.nw);
     }
     const size_t smem = gen_smem_bytes(B);
     cudaFuncSetAttribute(conn_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -419,19 +419,24 @@ __device__ __forceinline__ int pool_argmax(const snn_conn_t &C, const float *r, 
 
 // Final spikes of one neuron of one sample: traces (nodes.py:96-103), clamp / unclamp (network.py:415-429),
 // recordings, and (POOL) the next rate of every MaxPool2dConnection leaving the layer.  Returns the spike that is published.
+// (POOL) A PassThroughNodes layer has no traces (its forward never reaches Nodes.forward) and a float32 s.
 template <bool POOL>
 __device__ __forceinline__ bool finalize_neuron(const DevNet &N, const DevLayer &D, bool s, float xold, size_t k, int b, int j, int t, int wr,
                                                 int li) {
     const snn_layer_t &L = D.L;
+    const bool pass = POOL && L.kind == SNN_NODE_PASSTHROUGH;
     bool sf = s;
-    if (L.traces) {
+    if (L.traces && !pass) {
         const float x = trace_step(xold, s, L.trace_decay, L.trace_scale, L.traces_additive);
         L.x[k] = x;
         if (D.xpub) D.xpub[((size_t)wr * N.B + b) * L.n + j] = x;
     }
     if (L.clamp && L.clamp[(L.clamp_per_step ? (size_t)t * L.n : 0) + j]) sf = true;
     if (L.unclamp && L.unclamp[(L.unclamp_per_step ? (size_t)t * L.n : 0) + j]) sf = false;
-    if (t == N.T - 1) L.s[k] = sf ? 1 : 0;
+    if (t == N.T - 1) {
+        if (pass) ((float *)L.s)[k] = sf ? 1.0f : 0.0f;
+        else L.s[k] = sf ? 1 : 0;
+    }
     if (L.rec_s) L.rec_s[((size_t)t * N.B + b) * L.n + j] = sf ? 1 : 0;
     if (L.rec_count && sf) L.rec_count[k] += 1;
     if (POOL) pool_rate_step(N, li, k, t, sf);
@@ -581,7 +586,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
         for (int q = 0; q < 4; ++q) { fw[q] = fwn[q]; af[q] = afn[q]; }
         prefetch(b + SNN_GEN_WARPS);
         float v = 0.0f, rc = 0.0f, xold = 0.0f, ic = 0.0f;
-        if (valid) {
+        if (valid && !(POOL && L.kind == SNN_NODE_PASSTHROUGH)) {   // (PassThroughNodes: no v, refrac_count, traces)
             v = L.v[k];
             if (L.kind != SNN_NODE_MCP) rc = L.refrac_count[k];
             if (L.traces && !deferred) xold = L.x[k];
@@ -638,7 +643,11 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
             if (L.ext && !(N.one_step && has_in)) { bool nb = false; cur = cur + ld_ext(L, ((size_t)t * B + b) * n + j, nb); }
             if (L.inject_v) v = v + L.inject_v[(L.inject_per_step ? (size_t)t * n : 0) + j];  // network.py:398-404
             float xin = cur;
-            if (dc) {
+            const bool pass = POOL && L.kind == SNN_NODE_PASSTHROUGH;   // no v, refrac_count or summed of its own
+            if (pass) {   // PassThroughNodes.forward (conversion/nodes.py:137-144): s = x
+                s = xin != 0.0f;
+                nonbin |= s && xin != 1.0f;
+            } else if (dc) {
                 s = dc_step(L, v, rc, xin, theta);
                 if (L.has_lbound && v < L.lbound) v = L.lbound;  // nodes.py:1108-1109
             } else if (L.kind == SNN_NODE_IF) {
@@ -651,13 +660,17 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
             } else if (L.kind == SNN_NODE_MCP) {   // McCullochPitts.forward (nodes.py:278-288): voltages equal the inputs
                 v = xin;
                 s = v >= L.thresh;
+            } else if (POOL && L.kind == SNN_NODE_SUBIF) {
+                s = subif_step(L, v, rc, xin);
             } else {
                 s = lif_step(L, v, rc, xin);
             }
-            L.v[k] = v;
-            if (L.kind != SNN_NODE_MCP) L.refrac_count[k] = rc;
-            if (L.sum_input) L.summed[k] = L.summed[k] + xin;
-            if (L.rec_v) L.rec_v[((size_t)t * B + b) * n + j] = v;
+            if (!pass) {
+                L.v[k] = v;
+                if (L.kind != SNN_NODE_MCP) L.refrac_count[k] = rc;
+                if (L.sum_input) L.summed[k] = L.summed[k] + xin;
+                if (L.rec_v) L.rec_v[((size_t)t * B + b) * n + j] = v;
+            }
             cnt += s ? 1 : 0;
         }
         const uint32_t word = __ballot_sync(0xffffffffu, valid && s);
@@ -686,6 +699,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
     if (D.anyf && tile == 0)   // the flag slot of step t + 1 (last read in step t - 1)
         for (int b = b0 + threadIdx.x; b < b1; b += SNN_GEN_THREADS) D.anyf[(size_t)((t + 1) % 3) * B + b] = 0u;
 
+    if (POOL && nonbin && N.err) atomicOr(N.err, SNN_ERR_NONBINARY);   // a PassThroughNodes input outside {0, 1}
     // theta += theta_plus * sum_b s  (nodes.py:1093-1094)
     if (dc && L.learning && valid && cnt > 0) atomicAdd(D.thcnt + (size_t)(t % 3) * n + j, cnt);
     if (deferred && tile == 0) {

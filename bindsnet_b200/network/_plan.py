@@ -33,14 +33,20 @@ def _state(t: torch.Tensor, name: str, owner: str) -> torch.Tensor:
 
 def fill_layer(d: "_abi.SnnLayer", layer, name: str, B: int) -> None:
     layer._fill_desc(d)
-    if layer.s.dtype not in (torch.bool, torch.uint8) or tuple(layer.s.shape) != (B, *layer.shape):
+    if d.kind == _abi.SNN_NODE_PASSTHROUGH:
+        # PassThroughNodes.forward stores its float input as s (conversion/nodes.py:137-144): the kernel keeps it float32
+        if tuple(layer.s.shape) != (B, *layer.shape):
+            layer.s = torch.zeros(B, *layer.shape, dtype=torch.float32, device=layer.s.device)
+        elif layer.s.dtype != torch.float32:
+            layer.s = layer.s.float()
+    elif layer.s.dtype not in (torch.bool, torch.uint8) or tuple(layer.s.shape) != (B, *layer.shape):
         # Input.forward aliases user input into s in the reference (nodes.py:219); we keep a
         # private bool tensor of the canonical shape instead.
         layer.s = torch.zeros(B, *layer.shape, dtype=torch.bool, device=layer.s.device)
     if not layer.s.is_contiguous():
         layer.s = layer.s.contiguous()
     d.s = _ptr(_as_u8(layer.s))
-    if d.kind != _abi.SNN_NODE_INPUT:
+    if d.kind not in (_abi.SNN_NODE_INPUT, _abi.SNN_NODE_PASSTHROUGH):
         d.v = _ptr(_state(layer.v, "v", name))
         if d.kind != _abi.SNN_NODE_MCP:
             d.refrac_count = _ptr(_state(layer.refrac_count, "refrac_count", name))
@@ -103,6 +109,11 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
         raise TypeError("connection weights must be contiguous float32")
     if d.kind != _abi.SNN_CONN_CONV2D and tuple(w.shape) != (conn.source.n, conn.target.n):
         raise ValueError(f"weight shape {tuple(w.shape)} != ({conn.source.n}, {conn.target.n})")
+    if d.kind == _abi.SNN_CONN_CONV2D and tuple(conn.b.shape) != (d.cout,):
+        # F.conv2d's own error in the reference's first compute (topology.py:799-815); ann_to_snn makes such a bias for
+        # an nn.Conv2d without one (conversion.py:197-199)
+        raise RuntimeError(f"Given weight of size {list(w.shape)}, expected bias to be 1-dimensional with {d.cout} elements, "
+                           f"but got bias of size {list(conn.b.shape)} instead")
     d.w = _ptr(w)
     static = d.rule == _abi.SNN_RULE_NONE or (d.rule == _abi.SNN_RULE_NOOP and d.weight_decay in (0.0, 1.0))
     if static and not d.has_norm:
@@ -264,21 +275,49 @@ def build_net(
                 d.rec_v = _ptr(r[1]); keep.append(r[1])
             if len(r) > 2 and r[2] is not None:
                 d.rec_count = _ptr(r[2]); keep.append(r[2])
+        if d.kind == _abi.SNN_NODE_PASSTHROUGH and name in injects:
+            raise NotImplementedError(f"injects_v into {name!r}: a PassThroughNodes layer has no voltage of its own")
     masks = getattr(network, "_conn_masks", None) or {}
+    by_id = {id(layer): i for i, layer in enumerate(network.layers.values())}
     for i, ((src, tgt), conn) in enumerate(network.connections.items()):
         if network.learning and isinstance(conn, MaxPool2dConnection):
             raise AttributeError(conn._no_w_message())   # the reference fails in the first step's update
-        fill_conn(net.conns[i], conn, index[src], index[tgt], float(network.dt), B, network._rule_kwargs_of((src, tgt)))
+        # the source is the connection's own source layer (network.py:226-248 reads connection.source.s): ann_to_snn's
+        # keys name the previous ANN child, which need not be a layer
+        s_idx = by_id.get(id(conn.source), index.get(src))
+        if s_idx is None:
+            raise KeyError(f"the source of connection {(src, tgt)} is not a layer of the network")
+        fill_conn(net.conns[i], conn, s_idx, index[tgt], float(network.dt), B, network._rule_kwargs_of((src, tgt)))
         m = masks.get((src, tgt))
         if m is not None:
             net.conns[i].mask = _ptr(m)
             keep.append(m)
+        check_passthrough(net, i, type(conn).__name__)
     conns = [net.conns[i] for i in range(net.n_conns)]
-    if any(d.kind == _abi.SNN_CONN_MAXPOOL2D for d in conns) and any(
+    layers = [net.layers[i] for i in range(net.n_layers)]
+    if (any(d.kind == _abi.SNN_CONN_MAXPOOL2D for d in conns) or any(d.kind in CONVERSION_KINDS for d in layers)) and any(
             d.kind == _abi.SNN_CONN_SPARSE or d.f_prob or d.f_mask or d.f_int for d in conns):
-        raise NotImplementedError("a network with a MaxPool2dConnection and a SparseConnection or MulticompartmentConnection "
-                                  "features is not implemented by the CUDA core (each has its own instantiation of the window kernel)")
+        raise NotImplementedError("a network with a MaxPool2dConnection, SubtractiveResetIFNodes or PassThroughNodes and a "
+                                  "SparseConnection or MulticompartmentConnection features is not implemented by the CUDA core "
+                                  "(each has its own instantiation of the window kernel)")
     return net, keep
+
+
+CONVERSION_KINDS = (_abi.SNN_NODE_SUBIF, _abi.SNN_NODE_PASSTHROUGH)
+
+
+def check_passthrough(net: "_abi.SnnNet", i: int, what: str) -> None:
+    """A PassThroughNodes layer carries 0 / 1 spikes (include/snn_b200.h): refuse, before anything runs, a connection
+    into one that is not a MaxPool2dConnection (its input could take other values) and a learning rule other than NoOp
+    at either end."""
+    d = net.conns[i]
+    into, at = net.layers[d.tgt].kind == _abi.SNN_NODE_PASSTHROUGH, _abi.SNN_NODE_PASSTHROUGH in (net.layers[d.src].kind, net.layers[d.tgt].kind)
+    if into and d.kind != _abi.SNN_CONN_MAXPOOL2D:
+        raise NotImplementedError(f"a {what} into a PassThroughNodes layer is not implemented by the CUDA core (only "
+                                  "MaxPool2dConnection, whose output is 0 / 1 spikes)")
+    if at and d.rule not in (_abi.SNN_RULE_NONE, _abi.SNN_RULE_NOOP):
+        raise NotImplementedError(f"a learning rule other than NoOp on a {what} to or from a PassThroughNodes layer is not "
+                                  "implemented by the CUDA core")
 
 
 # ---- single-operator helpers ---------------------------------------------------------------

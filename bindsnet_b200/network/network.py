@@ -145,9 +145,9 @@ class Network(torch.nn.Module):
             if layers is not None and tgt not in layers:
                 continue
             if draw is not None and type(conn) is MulticompartmentConnection:
-                out = _plan.compute_single_connection(conn, self.layers[src].s, draw=(draw[0], draw[1], k))
+                out = _plan.compute_single_connection(conn, conn.source.s, draw=(draw[0], draw[1], k))
             else:
-                out = conn.compute(self.layers[src].s)
+                out = conn.compute(conn.source.s)
             out = out.view(B, *self.layers[tgt].shape).float()
             cur[tgt] = cur[tgt] + out if tgt in cur else out
         return cur
@@ -202,7 +202,7 @@ class Network(torch.nn.Module):
         for name, layer in self.layers.items():
             if mon.obj is layer:
                 ok = all(v in Monitor.FUSED_VARS for v in mon.state_vars)
-                ok = ok and not ("v" in mon.state_vars and layer.kind == _abi.SNN_NODE_INPUT)
+                ok = ok and not ("v" in mon.state_vars and layer.kind in (_abi.SNN_NODE_INPUT, _abi.SNN_NODE_PASSTHROUGH))
                 return name if ok else None
         return None
 
@@ -308,8 +308,9 @@ class Network(torch.nn.Module):
             if isinstance(mon, SpikeCounter):
                 continue
             rs, rv, _ = rec[lname]
-            if "s" in mon.state_vars:
-                mon._push_window("s", rs.view(torch.bool).view(T, B, *layer.shape))
+            if "s" in mon.state_vars:   # (a PassThroughNodes layer's s is float32)
+                rs = rs.float() if layer.kind == _abi.SNN_NODE_PASSTHROUGH else rs.view(torch.bool)
+                mon._push_window("s", rs.view(T, B, *layer.shape))
             if "v" in mon.state_vars:
                 mon._push_window("v", rv.view(T, B, *layer.shape))
 
@@ -369,9 +370,10 @@ class Network(torch.nn.Module):
         from ..learning import learning as L
         from ..learning import MCC_learning as ML
         from . import nodes as N, topology as Tp
+        from ..conversion import nodes as CN
 
         builtin_nodes = (N.Input, N.LIFNodes, N.DiehlAndCookNodes, N.IFNodes, N.CurrentLIFNodes, N.AdaptiveLIFNodes, N.BoostedLIFNodes,
-                         N.McCullochPitts)
+                         N.McCullochPitts, CN.SubtractiveResetIFNodes, CN.PassThroughNodes)
         for layer in self.layers.values():
             if type(layer) not in builtin_nodes and (layer.kind is None or type(layer).forward is not N.Nodes.forward):
                 return True

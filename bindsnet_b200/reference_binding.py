@@ -25,7 +25,8 @@ from . import _abi
 _KIND = {"Input": _abi.SNN_NODE_INPUT, "LIFNodes": _abi.SNN_NODE_LIF, "DiehlAndCookNodes": _abi.SNN_NODE_DC,
          "AdaptiveLIFNodes": _abi.SNN_NODE_DC,            # DiehlAndCookNodes.forward without the one-spike arbitration (nodes.py:921-946)
          "IFNodes": _abi.SNN_NODE_IF, "CurrentLIFNodes": _abi.SNN_NODE_CURRENT_LIF, "BoostedLIFNodes": _abi.SNN_NODE_BOOSTED_LIF,
-         "McCullochPitts": _abi.SNN_NODE_MCP}
+         "McCullochPitts": _abi.SNN_NODE_MCP,
+         "SubtractiveResetIFNodes": _abi.SNN_NODE_SUBIF, "PassThroughNodes": _abi.SNN_NODE_PASSTHROUGH}   # conversion/nodes.py
 
 
 def _f(x) -> float:
@@ -58,6 +59,16 @@ def fill_layer(d: "_abi.SnnLayer", layer, B: int, keep: List[torch.Tensor]) -> N
         d.x = layer.x.data_ptr()
     if layer.sum_input:
         d.summed = layer.summed.data_ptr()
+    if kind == _abi.SNN_NODE_PASSTHROUGH:
+        # PassThroughNodes.forward stores its float input as s (conversion/nodes.py:137-144); before its first step s is
+        # still the bool tensor of Nodes.set_batch_size: hand the core a float32 one with the same values
+        if tuple(layer.s.shape) != (B, *layer.shape):
+            layer.s = torch.zeros(B, *layer.shape, dtype=torch.float32, device=layer.s.device)
+        elif layer.s.dtype != torch.float32 or not layer.s.is_contiguous():
+            layer.s = layer.s.float().contiguous()
+        d.traces = d.sum_input = 0                                                        # its forward never reaches Nodes.forward
+        d.s = layer.s.data_ptr()
+        return
     # Input.forward aliases the caller's input into s (nodes.py:219): give the core a private bool tensor
     if layer.s.dtype not in (torch.bool, torch.uint8) or tuple(layer.s.shape) != (B, *layer.shape) or not layer.s.is_contiguous():
         layer.s = torch.zeros(B, *layer.shape, dtype=torch.bool, device=layer.s.device)
@@ -160,6 +171,11 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
             raise NotImplementedError(f"{type(conn).__name__} is outside the accelerated path")
         rule = conn.update_rule
         d.kind = _abi.SNN_CONN_DENSE
+        if not conn.w.is_sparse and not conn.w.is_contiguous():
+            # ann_to_snn hands nn.Linear weights over as weight.t() (conversion.py:177-180): stored contiguous in place,
+            # with the same values, since the core updates w in its own row-major storage
+            with torch.no_grad():
+                conn.w.data = conn.w.data.contiguous()
         w = conn.w
         d.has_norm = int(conn.norm is not None)                                           # topology.py:383-392: sum of |w|
         d.norm, d.norm_abs = (_f(conn.norm) if conn.norm is not None else 0.0), 1
@@ -226,6 +242,8 @@ def _fill_sparse(d: "_abi.SnnConn", conn, keep: List[torch.Tensor]) -> None:
 
 def build_net(network, inputs: Dict[str, torch.Tensor], T: int, B: int):
     """The window plan of a live reference ``Network`` (insertion orders: network.py:225, 386)."""
+    from .network._plan import check_passthrough
+
     net = _abi.SnnNet()
     net.abi_version = _abi.SNN_ABI_VERSION
     net.n_layers, net.n_conns = len(network.layers), len(network.connections)
@@ -244,12 +262,17 @@ def build_net(network, inputs: Dict[str, torch.Tensor], T: int, B: int):
             net.layers[i].ext_dtype = _abi.SNN_EXT_F32 if x.dtype == torch.float32 else _abi.SNN_EXT_U8
             keep.append(x)
     dev = next(iter(network.layers.values())).s.device
+    layers = list(network.layers.values())
     for i, ((s, t), conn) in enumerate(network.connections.items()):
         if network.learning and type(conn).__name__ == "MaxPool2dConnection":
             # the reference fails in the first step's update: learning.NoOp.update scales connection.w (learning.py:87-94)
             raise AttributeError("'MaxPool2dConnection' object has no attribute 'w' (run MaxPool2dConnection networks with "
                                  "learning off)")
-        fill_connection(net.conns[i], conn, names.index(s), names.index(t), float(network.dt), keep, B=B, device=dev)
+        # the source is connection.source (network.py:226-248): ann_to_snn's keys need not name it
+        src = next((k for k, layer in enumerate(layers) if layer is conn.source), None)
+        fill_connection(net.conns[i], conn, names.index(s) if src is None else src, names.index(t), float(network.dt), keep, B=B,
+                        device=dev)
+        check_passthrough(net, i, type(conn).__name__)
     return net, keep
 
 

@@ -49,6 +49,19 @@ extern "C" {
 #define SNN_NODE_CURRENT_LIF 4 /* CurrentLIFNodes nodes.py:681-826: decaying synaptic current i, gate taken after the decrement */
 #define SNN_NODE_BOOSTED_LIF 5 /* BoostedLIFNodes nodes.py:562-678: LIF without rest / reset / lbound: v *= decay, reset to 0 */
 #define SNN_NODE_MCP 6         /* McCullochPitts  nodes.py:231-305: v = x, s = v >= thresh; no refractory state (refrac_count NULL) */
+#define SNN_NODE_SUBIF 7       /* conversion.SubtractiveResetIFNodes conversion/nodes.py:73-99, one rounding per op:
+                                    v  = v + (rc == 0) * x          (-0.0 == 0 counts as 0)
+                                    rc = (rc > 0) * (rc - dt)       (rc <= 0 gives -0.0; 0 < rc < dt a negative rc, which
+                                                                     gates the NEXT step's input off)
+                                    s  = v >= thresh;  s ? rc = refrac, v = v - thresh   (reset by subtraction)
+                                    v  = max(v, lbound) if has_lbound;  then traces and summed += x as for every kind.
+                                  Generic tier only */
+#define SNN_NODE_PASSTHROUGH 8 /* conversion.PassThroughNodes conversion/nodes.py:137-144: s = x, nothing else (no trace or
+                                  summed update whatever the flags say; v and refrac_count are NULL).  `s` points to
+                                  FLOAT32 [B,n] holding 0.0 / 1.0 (the reference's s is the float input itself); a step whose
+                                  x is not in {0, 1} raises SNN_ERR_NONBINARY.  The only connection into such a layer is an
+                                  SNN_CONN_MAXPOOL2D, and a connection with such an endpoint has rule SNN_RULE_NONE or
+                                  SNN_RULE_NOOP.  Generic tier only */
 
 /* ---- connection kinds (reference: bindsnet/network/topology.py) ---- */
 #define SNN_CONN_DENSE 0 /* Connection: s.float() @ w + b                topology.py:332-346 */
@@ -119,7 +132,8 @@ extern "C" {
 #define SNN_ERR_UNSUPPORTED 2    /* valid reference configuration this build does not implement   */
 #define SNN_ERR_WORKSPACE 4      /* workspace too small                                           */
 #define SNN_ERR_CUDA 8           /* a CUDA runtime call failed                                    */
-#define SNN_ERR_NONBINARY 16     /* (device flag) an Input layer received a value outside {0,1}   */
+#define SNN_ERR_NONBINARY 16     /* (device flag) an Input layer received, or an SNN_NODE_PASSTHROUGH layer held or
+                                    received, a value outside {0,1} (spikes are carried as bits)    */
 #define SNN_ERR_BARRIER 32       /* (device flag) grid barrier timed out — kernel bailed out      */
 #define SNN_ERR_STRUCTURE 64     /* (device flag) a weight matrix does not have the structure its SNN_W_* hint claims */
 
@@ -145,7 +159,8 @@ typedef struct snn_layer {
     int32_t unclamp_per_step;
     int32_t inject_per_step;
     /* --- state, updated in place; shapes as in the reference --- */
-    uint8_t *s;          /* [B,n] 0/1.  in: spikes of step -1, out: spikes of step T-1      */
+    uint8_t *s;          /* [B,n] 0/1.  in: spikes of step -1, out: spikes of step T-1      
+                            (SNN_NODE_PASSTHROUGH: float32 0.0 / 1.0)                         */
     float *v;            /* [B,n]  (LIF, DC)                                                */
     float *refrac_count; /* [B,n]  (LIF, DC)                                                */
     float *x;            /* [B,n]  if traces                                                */

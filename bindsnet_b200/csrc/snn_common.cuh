@@ -97,8 +97,9 @@ struct DevNet {
     int32_t sp_units;             // sparse gather units of a step (0: the plan has no SparseConnection)
     DevSparse sp[SNN_MAX_CONNS];
     int32_t any_feat;             // some MCC connection carries Probability / Mask / Intensity features
-    int32_t any_pool;             // some connection is a MaxPool2dConnection (SNN_CONN_MAXPOOL2D), or some layer is an
-                                  // SNN_NODE_SUBIF / SNN_NODE_PASSTHROUGH one: the plan runs the POOL instantiation
+    int32_t any_pool;             // some connection is a MaxPool2dConnection (SNN_CONN_MAXPOOL2D) or a LocalConnection2D
+                                  // (SNN_CONN_LOCAL2D), or some layer is an SNN_NODE_SUBIF / SNN_NODE_PASSTHROUGH one: the
+                                  // plan runs the POOL instantiation
     float *pool_r1[SNN_MAX_CONNS];   // MaxPool2dConnection: the workspace slot of its rates (pool_rate_slot)
 };
 
@@ -124,6 +125,17 @@ static inline int snn_pool_geometry_ok(const snn_conn_t &C, int n_src, int n_tgt
         for (int k = 0; k < C.kw && !any; ++k) any = o * C.sw - C.pw + k * C.dw >= 0 && o * C.sw - C.pw + k * C.dw < C.win;
         if (!any) return SNN_ERR_BAD_ARG;
     }
+    return SNN_OK;
+}
+
+// A LocalConnection2D's geometry (snn_b200.h): the layer sizes, the reference's output size int((hin - kh) / sh) + 1 of
+// a window that fits, no padding or dilation, w present and no bias.
+static inline int snn_local2d_geometry_ok(const snn_conn_t &C, int n_src, int n_tgt) {
+    if (!C.w || C.b) return SNN_ERR_BAD_ARG;
+    if (C.cin < 1 || C.cout < 1 || C.kh < 1 || C.kw < 1 || C.sh < 1 || C.sw < 1) return SNN_ERR_BAD_ARG;
+    if (C.ph != 0 || C.pw != 0 || C.dh != 1 || C.dw != 1 || C.kh > C.hin || C.kw > C.win) return SNN_ERR_BAD_ARG;
+    if (C.hout != (C.hin - C.kh) / C.sh + 1 || C.wout != (C.win - C.kw) / C.sw + 1) return SNN_ERR_BAD_ARG;
+    if ((long long)C.cin * C.hin * C.win != n_src || (long long)C.cout * C.hout * C.wout != n_tgt) return SNN_ERR_BAD_ARG;
     return SNN_OK;
 }
 

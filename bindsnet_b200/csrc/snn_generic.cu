@@ -1,6 +1,6 @@
 // snn_generic.cu — generic persistent window kernel (any topology of Input / McCullochPitts / IF / LIF / BoostedLIF /
-// CurrentLIF / DiehlAndCook / SubtractiveResetIF / PassThrough populations joined by dense, convolutional, sparse and
-// pooling connections).
+// CurrentLIF / DiehlAndCook / SubtractiveResetIF / PassThrough populations joined by dense, convolutional, sparse,
+// pooling and 2-D locally connected connections).
 //
 // One cooperative grid iterates the whole T-step window of Network.run (reference:
 // bindsnet/network/network.py:380-465) with at most four grid barriers per step and no host involvement.
@@ -14,7 +14,7 @@
 //   phase 2  one_spike layers, same units: resolve the winner per sample, final spikes, traces
 //   barrier
 //   phase 3  unit = (connection, 32-column tile, chunk of source rows): STDP + decay + clamp
-//            (learning.py / MCC_learning.py); dense MSTDP by source tiles; conv rules spread over the grid
+//            (learning.py / MCC_learning.py); dense MSTDP by source tiles; conv and local rules spread over the grid
 //   barrier  (+ masks + barrier when Network.run got masks)
 // With a SparseConnection (the <CTAS, true> instantiation): a window pre-pass builds the column-block tables of the
 // patterns, and every step starts with the sparse gather (unit = (connection, column block, sample chunk)) and a
@@ -53,9 +53,11 @@ __device__ __forceinline__ void sparse_unit(const DevNet &N, int u, int &c, int 
 // code (and register allocation) is exactly what it is without the feature.
 // FEAT: the plan holds a MulticompartmentConnection with Probability / Mask / Intensity features (snn_b200.h); only the
 // dense gather of phase 1 differs.  The two are not combined in one plan.
-// POOL: the plan holds a MaxPool2dConnection or a layer of ann_to_snn's kinds (SNN_NODE_SUBIF, SNN_NODE_PASSTHROUGH, whose
-// s is float32): phase 1 gathers the pooled spikes and steps those layers, and every finalised spike of a pooling source
-// advances its rates (pool_rate_step); the prologue writes the rates of step 0.  Not combined with SPARSE or FEAT.  The
+// POOL: the plan holds a MaxPool2dConnection, a LocalConnection2D or a layer of ann_to_snn's kinds (SNN_NODE_SUBIF,
+// SNN_NODE_PASSTHROUGH, whose s is float32): phase 1 gathers the pooled spikes and the local receptive fields and steps
+// those layers, the learning phase runs the local rules over the grid, normalize() scales the local rows, and every
+// finalised spike of a pooling source advances its rates (pool_rate_step); the prologue writes the rates of step 0.  Not
+// combined with SPARSE or FEAT.  The
 // barriers are those of the plain window: the rates a gather reads were written before the barrier that ends the previous
 // step (or, in one-step mode, before the barrier that ends the source layer).
 template <int CTAS, bool SPARSE, bool FEAT, bool POOL>
@@ -194,6 +196,7 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
             GPROF(4)
             for (int c = 0; c < N.n_conns; ++c) {
                 if (N.conns[c].kind == SNN_CONN_CONV2D && N.conns[c].rule != SNN_RULE_NONE) phase3_conv(N, c, blockIdx.x, G, t, M);
+                if (POOL && N.conns[c].kind == SNN_CONN_LOCAL2D && N.conns[c].rule != SNN_RULE_NONE) phase3_local2d(N, c, blockIdx.x, G, t);
                 if (SPARSE && N.conns[c].kind == SNN_CONN_SPARSE) decay_sparse(N.conns[c], blockIdx.x, G);
             }
             GPROF(5)
@@ -232,6 +235,8 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
             for (int c = 0; c < N.n_conns; ++c)
                 if (N.conns[c].tgt == li && N.conns[c].has_norm) {
                     if (N.conns[c].kind == SNN_CONN_CONV2D) normalize_conv_item(N.conns[c], tile, N.layers[li].nw);
+                    else if (POOL && N.conns[c].kind == SNN_CONN_LOCAL2D)
+                        normalize_local2d_item(N.conns[c], N.conns[c].cin * N.layers[li].L.n, tile, N.layers[li].nw);
                     else normalize_tile(N.conns[c], N.layers[N.conns[c].src].L.n, N.layers[li].L.n, tile, M.red);
                 }
         }
@@ -256,8 +261,9 @@ static int plan_units(DevNet &N, int cap) {
         const snn_conn_t &C = N.conns[c];
         N.p3_first[c] = p3;
         N.p3_rc[c] = 0;
-        if (!N.learning || C.rule == SNN_RULE_NONE || C.kind == SNN_CONN_CONV2D || C.kind == SNN_CONN_SPARSE || C.kind == SNN_CONN_MAXPOOL2D)
-            continue;   // (a MaxPool2dConnection has no weights to update)
+        if (!N.learning || C.rule == SNN_RULE_NONE || C.kind == SNN_CONN_CONV2D || C.kind == SNN_CONN_SPARSE || C.kind == SNN_CONN_MAXPOOL2D ||
+            C.kind == SNN_CONN_LOCAL2D)
+            continue;   // (a MaxPool2dConnection has no weights to update; conv and local rules are spread over the grid)
         const int nwS = N.layers[C.src].nw, nwT = N.layers[C.tgt].nw;
         if (SNN_RULE_IS_MSTDP(C.rule)) { N.p3_rc[c] = 1; p3 += nwS; continue; }
         int rc = ceil_div(cap, nwT);
@@ -281,7 +287,8 @@ static int plan_units(DevNet &N, int cap) {
     if (spu > units) units = spu;
     bool conv_rule = false;
     for (int c = 0; c < N.n_conns; ++c)
-        if (N.learning && N.conns[c].kind == SNN_CONN_CONV2D && N.conns[c].rule != SNN_RULE_NONE) conv_rule = true;
+        if (N.learning && (N.conns[c].kind == SNN_CONN_CONV2D || N.conns[c].kind == SNN_CONN_LOCAL2D) && N.conns[c].rule != SNN_RULE_NONE)
+            conv_rule = true;
     int grid = conv_rule ? cap : (int)(units < cap ? units : cap);
     return grid < 1 ? 1 : grid;
 }
@@ -309,7 +316,7 @@ int snn_generic_launch(DevNet &N, cudaStream_t stream) {
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const size_t smem = snn_generic_smem_bytes(N.B);
     // two CTAs per SM unless SNN_B200_GVAR=3 asks for the spilling three-CTA experiment (plans without a SparseConnection,
-    // MCC features or a MaxPool2dConnection)
+    // MCC features or the POOL instantiation's kinds)
     const bool sparse = std::any_of(N.conns, N.conns + N.n_conns, [](const snn_conn_t &C) { return C.kind == SNN_CONN_SPARSE; });
     bool three = false;
     if (const char *v = getenv("SNN_B200_GVAR")) three = !sparse && !N.any_feat && !N.any_pool && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;

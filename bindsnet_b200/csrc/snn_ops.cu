@@ -134,6 +134,36 @@ __global__ void __launch_bounds__(256) pool_compute_kernel(snn_conn_t C, int ns,
 
 __global__ void __launch_bounds__(SNN_GEN_THREADS) conv_normalize_kernel(snn_conn_t C) { normalize_conv_item(C, blockIdx.x, gridDim.x); }
 
+// LocalConnection2D.compute (topology.py:1717-1740) on byte spikes: the window gather's gather_local2d order (k ascending
+// within a channel from +0, then the channels).  Thread = one target neuron of one sample.
+__global__ void __launch_bounds__(256) local2d_compute_kernel(snn_conn_t C, int ns, int nt, int B, const uint8_t *__restrict__ s,
+                                                              float *__restrict__ out) {
+    const size_t total = (size_t)B * nt;
+    const int K = C.kh * C.kw, P = C.hout * C.wout;
+    for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+        const int b = (int)(e / nt), j = (int)(e - (size_t)b * nt), l = j % P, oy = l / C.wout, ox = l - oy * C.wout;
+        const uint8_t *sb = s + (size_t)b * ns;
+        float p = 0.0f;
+        for (int ci = 0; ci < C.cin; ++ci) {
+            const float *wr = C.w + ((size_t)ci * nt + j) * K;
+            float q = 0.0f;
+            for (int ky = 0; ky < C.kh; ++ky)
+                for (int kx = 0; kx < C.kw; ++kx)
+                    if (sb[(ci * C.hin + oy * C.sh + ky) * C.win + ox * C.sw + kx]) q = q + wr[ky * C.kw + kx];
+            p = p + q;
+        }
+        out[e] = p;
+    }
+}
+
+__global__ void __launch_bounds__(SNN_GEN_THREADS) local2d_normalize_kernel(snn_conn_t C, int rows) {
+    normalize_local2d_item(C, rows, blockIdx.x, gridDim.x);
+}
+
+__global__ void __launch_bounds__(SNN_GEN_THREADS) local2d_update_kernel(const __grid_constant__ DevNet N, int ci) {
+    phase3_local2d(N, ci, blockIdx.x, gridDim.x, 0);
+}
+
 // bit-pack the CURRENT spikes of the two layers of a connection into slot 0 (F32: a PassThroughNodes layer's float32 s)
 template <bool F32>
 __global__ void pack_bits_kernel(const uint8_t *__restrict__ s, uint32_t *__restrict__ bits, int B, int n, int nw) {
@@ -225,6 +255,14 @@ int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, 
                    B, s, out);
         return cuda_rc(cudaGetLastError());
     }
+    if (conn->kind == SNN_CONN_LOCAL2D) {
+        const int rc = snn_local2d_geometry_ok(*conn, n_src, n_tgt);
+        if (rc != SNN_OK) return rc;
+        const size_t total = (size_t)B * n_tgt;
+        const int blocks = (int)((total + 255) / 256 < 4736 ? (total + 255) / 256 : 4736);
+        SNN_LAUNCH(local2d_compute_kernel, blocks, 256, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
+        return cuda_rc(cudaGetLastError());
+    }
     if (conn->kind == SNN_CONN_CONV2D) {
         if (!conn->b || conn->cin * conn->hin * conn->win != n_src || conn->cout * conn->hout * conn->wout != n_tgt) return SNN_ERR_BAD_ARG;
         const size_t total = (size_t)B * n_tgt;
@@ -262,9 +300,15 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
     if (!C.w) return SNN_ERR_BAD_ARG;
     const bool pass = net->layers[C.src].kind == SNN_NODE_PASSTHROUGH || net->layers[C.tgt].kind == SNN_NODE_PASSTHROUGH;
     if (pass && C.rule != SNN_RULE_NONE && C.rule != SNN_RULE_NOOP) return SNN_ERR_UNSUPPORTED;   // (snn_b200.h)
-    // the single-operator update is the dense [n_src, n_tgt] rule application; convolutional weights and the
-    // reward-modulated rules (whose state lives in the window plan) are only updated inside run_window
-    if (C.kind != SNN_CONN_DENSE && C.kind != SNN_CONN_MCC) return SNN_ERR_UNSUPPORTED;
+    // the single-operator update is the dense [n_src, n_tgt] rule application or a LocalConnection2D's; convolutional
+    // weights and the reward-modulated rules (whose state lives in the window plan) are only updated inside run_window
+    const bool local = C.kind == SNN_CONN_LOCAL2D;
+    if (C.kind != SNN_CONN_DENSE && C.kind != SNN_CONN_MCC && !local) return SNN_ERR_UNSUPPORTED;
+    if (local) {
+        const int rc = snn_local2d_geometry_ok(C, net->layers[C.src].n, net->layers[C.tgt].n);
+        if (rc != SNN_OK) return rc;
+        if (C.rule == SNN_RULE_MCC_POSTPRE) return SNN_ERR_UNSUPPORTED;
+    }
     if (SNN_RULE_IS_MSTDP(C.rule)) return SNN_ERR_UNSUPPORTED;
     if (C.rule == SNN_RULE_NONE) return SNN_OK;
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -288,6 +332,12 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
         if (D.L.kind == SNN_NODE_PASSTHROUGH) SNN_LAUNCH(pack_bits_kernel<true>, (warps * 32 + 255) / 256, 256, 0, stream, D.L.s, D.bits, B, D.L.n, D.nw);
         else SNN_LAUNCH(pack_bits_kernel<false>, (warps * 32 + 255) / 256, 256, 0, stream, D.L.s, D.bits, B, D.L.n, D.nw);
     }
+    if (local) {   // dense over w, spread over the grid like the window's learning phase
+        const size_t NW = (size_t)N.layers[C.tgt].L.n * C.cin * C.kh * C.kw;
+        const int blocks = (int)((NW + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS < 1184 ? (NW + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS : 1184);
+        SNN_LAUNCH(local2d_update_kernel, blocks, SNN_GEN_THREADS, 0, stream, N, ci);
+        return cuda_rc(cudaGetLastError());
+    }
     const size_t smem = gen_smem_bytes(B);
     cudaFuncSetAttribute(conn_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     SNN_LAUNCH(conn_update_kernel, N.layers[C.tgt].nw, SNN_GEN_THREADS, smem, stream, N, ci);
@@ -299,6 +349,11 @@ int snn_b200_conn_normalize(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt
     if (conn->kind == SNN_CONN_SPARSE) return SNN_ERR_UNSUPPORTED;   // the reference's normalize fails on a sparse w too
     if (!conn->w) return SNN_ERR_BAD_ARG;
     if (!conn->has_norm) return SNN_OK;
+    if (conn->kind == SNN_CONN_LOCAL2D) {   // rows of w viewed as [cin * n_tgt, K]
+        const int rows = conn->cin * n_tgt;
+        SNN_LAUNCH(local2d_normalize_kernel, (rows + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, rows);
+        return cuda_rc(cudaGetLastError());
+    }
     if (conn->kind == SNN_CONN_CONV2D) {
         const int F = conn->cout * conn->cin;
         SNN_LAUNCH(conv_normalize_kernel, (F + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn);

@@ -373,6 +373,39 @@ __device__ __forceinline__ float gather_conv(const snn_conn_t &C, const uint32_t
     return p + C.b[co];
 }
 
+// LocalConnection2D.compute (topology.py:1717-1740) for target neuron j = (f, oy, ox) of one sample (n target neurons):
+// per input channel the sum of its own weights w[ci, j, k] whose window position k spiked (k ascending, from +0), then
+// the channel sums in ascending ci (the reference's sum(-1).sum(1)).  The kw window bits of a kernel row are cut out of
+// the bit row 32 at a time, as in gather_conv.  The weights are read where they are: a lane walks its own contiguous row
+// w[ci, j, :] (K floats), so the set bits of one row land in the same 32-byte sectors.  A weight under a silent input is
+// never read, which differs from the reference's s_unfold * w for a non-finite weight (DESIGN.md section 8).
+template <bool STAGED_BITS>
+__device__ __forceinline__ float gather_local2d(const snn_conn_t &C, const uint32_t *sb, int n, int j, bool valid) {
+    if (!valid) return 0.0f;
+    const int K = C.kh * C.kw, P = C.hout * C.wout, l = j % P, oy = l / C.wout, ox = l - oy * C.wout;
+    float p = 0.0f;
+    for (int ci = 0; ci < C.cin; ++ci) {
+        const float *wr = C.w + ((size_t)ci * n + j) * K;
+        float q = 0.0f;
+        for (int ky = 0; ky < C.kh; ++ky) {
+            const int row = (ci * C.hin + oy * C.sh + ky) * C.win + ox * C.sw;
+            for (int kx0 = 0; kx0 < C.kw; kx0 += 32) {
+                const int cnt = min(32, C.kw - kx0), bit0 = row + kx0, w0 = bit0 >> 5, sft = bit0 & 31;
+                const uint32_t lo = STAGED_BITS ? sb[w0] : __ldcg(sb + w0);
+                const uint32_t hi = sft + cnt > 32 ? (STAGED_BITS ? sb[w0 + 1] : __ldcg(sb + w0 + 1)) : 0u;
+                uint32_t bits = __funnelshift_r(lo, hi, sft) & (cnt >= 32 ? 0xffffffffu : ((1u << cnt) - 1u));
+                while (bits) {
+                    const int k = ky * C.kw + kx0 + __ffs(bits) - 1;
+                    bits &= bits - 1;
+                    q = q + __ldcg(wr + k);
+                }
+            }
+        }
+        p = p + q;
+    }
+    return p;
+}
+
 // ---------------------------------------------------------------------------------------
 // MaxPool2dConnection (SNN_CONN_MAXPOOL2D, topology.py:1124-1211).
 //
@@ -515,12 +548,13 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
     }
     int cnt = 0;  // candidates of this column over this warp's samples
 
-    // a convolutional input: stage the chunk's source bit rows and the taps of this tile's output channels
+    // a convolutional input: stage the chunk's source bit rows and the taps of this tile's output channels (POOL: a
+    // LocalConnection2D input gets its bit rows staged the same way; its weights are per target, not taps)
     int conv_c = -1, conv_slot = 0, co_base = 0;
     bool st_bits = false, st_taps = false;
     ConvGeo geo = {};
     for (int c = 0; c < N.n_conns && conv_c < 0; ++c)
-        if (N.conns[c].tgt == li && N.conns[c].kind == SNN_CONN_CONV2D) conv_c = c;
+        if (N.conns[c].tgt == li && (N.conns[c].kind == SNN_CONN_CONV2D || (POOL && N.conns[c].kind == SNN_CONN_LOCAL2D))) conv_c = c;
     if (conv_c >= 0) {
         const snn_conn_t &C = N.conns[conv_c];
         const DevLayer &S = N.layers[C.src];
@@ -532,7 +566,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
         co_base = (tile * SNN_TILE) / Lhw;
         const int co_hi = min(n - 1, tile * SNN_TILE + SNN_TILE - 1) / Lhw;
         const int ntaps = (co_hi - co_base + 1) * K;
-        st_taps = ntaps <= SNN_CONV_STAGE_TAPS;
+        st_taps = ntaps <= SNN_CONV_STAGE_TAPS && (!POOL || C.kind == SNN_CONN_CONV2D);
         if (st_bits) {
             const uint32_t *src = S.bits + ((size_t)conv_slot * B + b0) * S.nw;
             for (int k0 = threadIdx.x; k0 < words; k0 += 4 * SNN_GEN_THREADS) {
@@ -568,7 +602,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
         for (int q = 0; q < 4; ++q) {
             fwn[q] = 0u; afn[q] = 1u;
             if (q < ncl && b < b1 && N.conns[cl[q]].kind != SNN_CONN_CONV2D && !(SPARSE && N.conns[cl[q]].kind == SNN_CONN_SPARSE) &&
-                !(POOL && N.conns[cl[q]].kind == SNN_CONN_MAXPOOL2D)) {
+                !(POOL && (N.conns[cl[q]].kind == SNN_CONN_MAXPOOL2D || N.conns[cl[q]].kind == SNN_CONN_LOCAL2D))) {
                 const snn_conn_t &C = N.conns[cl[q]];
                 const DevLayer &S = N.layers[C.src];
                 const int slot = (N.one_step && C.src < li) ? wr : rd;
@@ -625,6 +659,9 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
                 const uint32_t *sb = S.bits + ((size_t)slot * B + b) * S.nw;
                 const int i = valid ? pool_argmax(C, r, j) : 0;
                 p = (valid && ((__ldcg(sb + (i >> 5)) >> (i & 31)) & 1u)) ? 1.0f : 0.0f;
+            } else if (POOL && C.kind == SNN_CONN_LOCAL2D) {
+                p = c == conv_c && st_bits ? gather_local2d<true>(C, M.cbits + (size_t)(b - b0) * S.nw, n, j, valid)
+                                           : gather_local2d<false>(C, S.bits + ((size_t)slot * B + b) * S.nw, n, j, valid);
             } else if (SPARSE && C.kind == SNN_CONN_SPARSE) {   // gathered by phase_sparse ahead of this phase
                 p = valid ? __ldcg(N.sp[c].out + (size_t)b * n + j) : 0.0f;
                 if (C.b && valid) p = p + C.b[j];
@@ -1163,6 +1200,67 @@ struct BitIter {
     }
 };
 
+// One weight of PostPre / WeightDependentPostPre / Hebbian from its batch-reduced pre / post terms U / V, then the base
+// class's decay and clamp (learning.py:457-497, 920-975, 1348-1380 on Conv2dConnection; :258-320, 717-791, 1186-1250 on
+// LocalConnection2D; :87-104).  A term is applied when its nu is non-zero (Hebbian: always).
+__device__ __forceinline__ float stdp_rule_apply(const snn_conn_t &C, float x, float U, float V, bool pre_on, bool post_on) {
+    if (C.rule == SNN_RULE_WDEP_POSTPRE) {
+        float upd = 0.0f;
+        if (pre_on) upd = upd - (C.nu0 * U) * (x - C.wmin);
+        if (post_on) upd = upd + (C.nu1 * V) * (C.wmax - x);
+        x = x + upd;
+    } else if (C.rule == SNN_RULE_HEBBIAN) {
+        x = x + C.nu0 * U;
+        x = x + C.nu1 * V;
+    } else {
+        if (pre_on) x = x - C.nu0 * U;
+        if (post_on) x = x + C.nu1 * V;
+    }
+    if (C.weight_decay != 0.0f) x = x * C.weight_decay;
+    if (C.has_clamp) x = clampf(x, C.wmin, C.wmax);
+    return x;
+}
+
+// The source neuron of element (n', m) of a LocalConnection2D rule (snn_b200.h): the unfolded source at flat position
+// (n' % P) * cin * K + m in [cin, P, K] order.
+__host__ __device__ __forceinline__ int local2d_rule_source(const snn_conn_t &C, int n, int m) {
+    const int K = C.kh * C.kw, P = C.hout * C.wout;
+    const int q = (n % P) * C.cin * K + m, ci = q / (P * K), r = q - ci * P * K, l = r / K, k = r - l * K;
+    const int oy = l / C.wout, ox = l - oy * C.wout, ky = k / C.kw, kx = k - ky * C.kw;
+    return (ci * C.hin + oy * C.sh + ky) * C.win + ox * C.sw + kx;
+}
+
+// PostPre / WeightDependentPostPre / Hebbian on a LocalConnection2D (learning.py:258-320, 717-791, 1186-1250), and the
+// decay of learning.NoOp.  Dense over w and spread over the grid (cta of ncta): element e = n' * cin * K + m takes
+//   U = reduce_b x_tgt[b, n'] * s_src[b, src],  V = reduce_b s_tgt[b, n'] * x_src[b, src]   (src = local2d_rule_source)
+// with the batch sum in ascending b, the terms of the silent samples skipped (they are exact zeros).  Traces are read
+// from the layers' own arrays, framed by the grid barriers around the learning phase.  Every element is rewritten every
+// step: the decay and the clamp reach all of w, and at B = 128 nearly every receptive field holds a pre-synaptic spike.
+__device__ void phase3_local2d(const DevNet &N, int ci_, int cta, int ncta, int t) {
+    const snn_conn_t &C = N.conns[ci_];
+    const DevLayer &S = N.layers[C.src], &G = N.layers[C.tgt];
+    const int B = N.B, ns = S.L.n, nt = G.L.n, Mw = C.cin * C.kh * C.kw;
+    const size_t NW = (size_t)nt * Mw, start = (size_t)cta * SNN_GEN_THREADS + threadIdx.x, stride = (size_t)ncta * SNN_GEN_THREADS;
+    if (!SNN_RULE_IS_STDP(C.rule)) {   // learning.NoOp: w *= weight_decay (learning.py:93-94), no clamp
+        if (C.weight_decay != 0.0f)
+            for (size_t e = start; e < NW; e += stride) C.w[e] = __ldcg(C.w + e) * C.weight_decay;
+        return;
+    }
+    const bool hebb = C.rule == SNN_RULE_HEBBIAN;
+    const bool pre_on = C.nu0 != 0.0f || hebb, post_on = C.nu1 != 0.0f || hebb;
+    const int wr = t & 1;
+    for (size_t e = start; e < NW; e += stride) {
+        const int n = (int)(e / Mw), src = local2d_rule_source(C, n, (int)(e - (size_t)n * Mw));
+        float U = 0.0f, V = 0.0f;
+        for (int b = 0; b < B; ++b) {
+            if (pre_on && bit_of(S.bits + ((size_t)wr * B + b) * S.nw, src)) U = U + __ldcg(G.L.x + (size_t)b * nt + n);
+            if (post_on && bit_of(G.bits + ((size_t)wr * B + b) * G.nw, n)) V = V + __ldcg(S.L.x + (size_t)b * ns + src);
+        }
+        if (C.reduction == SNN_REDUCE_MEAN) { U = U / (float)B; V = V / (float)B; }
+        C.w[e] = stdp_rule_apply(C, __ldcg(C.w + e), U, V, pre_on, post_on);
+    }
+}
+
 // learning.MSTDP._conv2d_connection_update (learning.py:1942-2015) with a per-sample eligibility
 // (SURVEY.md §0.8), PostPre / WeightDependentPostPre / Hebbian on a Conv2dConnection, and the decay-only
 // update of a conv connection without a rule (learning.NoOp).  Called once per CTA and step: every loop is
@@ -1204,22 +1302,7 @@ __device__ void phase3_conv(const DevNet &N, int ci_, int cta, int ncta, int t, 
                 U = U + u1; V = V + v1;
             }
             if (C.reduction == SNN_REDUCE_MEAN) { U = U / (float)B; V = V / (float)B; }
-            float x = __ldcg(C.w + e);
-            if (C.rule == SNN_RULE_WDEP_POSTPRE) {
-                float upd = 0.0f;
-                if (pre_on) upd = upd - (C.nu0 * U) * (x - C.wmin);
-                if (post_on) upd = upd + (C.nu1 * V) * (C.wmax - x);
-                x = x + upd;
-            } else if (hebb) {
-                x = x + C.nu0 * U;
-                x = x + C.nu1 * V;
-            } else {
-                if (pre_on) x = x - C.nu0 * U;
-                if (post_on) x = x + C.nu1 * V;
-            }
-            if (C.weight_decay != 0.0f) x = x * C.weight_decay;
-            if (C.has_clamp) x = clampf(x, C.wmin, C.wmax);
-            C.w[e] = x;
+            C.w[e] = stdp_rule_apply(C, __ldcg(C.w + e), U, V, pre_on, post_on);
         }
         return;
     }
@@ -1458,6 +1541,20 @@ __device__ void normalize_conv_item(const snn_conn_t &C, int tile, int ntiles) {
         for (int k = 0; k < KK; ++k) tot = tot + C.w[(size_t)f * KK + k];
         const float fac = C.norm / tot;
         for (int k = 0; k < KK; ++k) C.w[(size_t)f * KK + k] = C.w[(size_t)f * KK + k] * fac;
+    }
+}
+
+// LocalConnection2D.normalize (topology.py:1748-1759): w viewed as [cin * n, K], every row scaled by norm / its sum (sum in
+// ascending k; `norm / sum` is torch's reciprocal(sum) * norm).  No guard against a zero sum, like the reference: such a row
+// becomes inf / NaN.
+__device__ void normalize_local2d_item(const snn_conn_t &C, int rows, int tile, int ntiles) {
+    const int K = C.kh * C.kw;
+    for (int r = tile * SNN_GEN_THREADS + threadIdx.x; r < rows; r += ntiles * SNN_GEN_THREADS) {
+        float *w = C.w + (size_t)r * K;
+        float tot = 0.0f;
+        for (int k = 0; k < K; ++k) tot = tot + w[k];
+        const float fac = (1.0f / tot) * C.norm;
+        for (int k = 0; k < K; ++k) w[k] = w[k] * fac;
     }
 }
 

@@ -1,6 +1,7 @@
 """Learning rules for ``Connection`` — host-side mirror of ``bindsnet/learning/learning.py``
 (``LearningRule`` :25-104, ``NoOp`` :107-146, ``PostPre`` :149-420 / :457-497 (conv2d),
-``WeightDependentPostPre`` :562-653 / :920-975, ``Hebbian`` :1052-1136 / :1348-1380, ``MSTDP``).  The rule objects hold hyper-parameters; the update
+``WeightDependentPostPre`` :562-653 / :920-975, ``Hebbian`` :1052-1136 / :1348-1380, ``MSTDP``; the three unsupervised
+rules also on ``LocalConnection2D``, :258-320 / :717-791 / :1186-1250).  The rule objects hold hyper-parameters; the update
 itself is fused into the CUDA window kernels (``Network.run``) or submitted for one step by
 ``rule.update()``."""
 from __future__ import annotations
@@ -93,11 +94,12 @@ class LearningRule(ABC):
 
 
 def _check_connection(rule, connection) -> None:
-    """The STDP-family rules exist for ``Connection`` (``_connection_update``) and ``Conv2dConnection``
-    (``_conv2d_connection_update``); the reference's im2col ignores dilation, so a dilated filter is refused."""
-    from ..network.topology import Connection, Conv2dConnection
+    """The STDP-family rules exist for ``Connection`` (``_connection_update``), ``Conv2dConnection``
+    (``_conv2d_connection_update``) and ``LocalConnection2D`` (``_local_connection2d_update``); the reference's im2col
+    ignores dilation, so a dilated filter is refused."""
+    from ..network.topology import Connection, Conv2dConnection, LocalConnection2D
 
-    if not isinstance(connection, (Connection, Conv2dConnection)):
+    if not isinstance(connection, (Connection, Conv2dConnection, LocalConnection2D)):
         raise NotImplementedError("This learning rule is not supported for this Connection type.")
     if isinstance(connection, Conv2dConnection) and connection._geometry[3] != (1, 1):
         raise NotImplementedError(f"{type(rule).__name__} on a dilated Conv2dConnection is undefined in the reference (im2col ignores dilation)")

@@ -11,7 +11,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from .. import _abi, _backend
-from .topology import MaxPool2dConnection
+from .topology import LocalConnection2D, MaxPool2dConnection
 
 
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
@@ -99,6 +99,13 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
         conn._fill_desc(d, dt, rule)
         return
     conn._fill_desc(d, dt, rule)
+    if d.kind == _abi.SNN_CONN_LOCAL2D:   # [cin, n, K] weights, no bias (topology.py:1717-1740 never reads b)
+        w = conn.w
+        if w.dtype != torch.float32 or not w.is_contiguous():
+            raise TypeError("connection weights must be contiguous float32")
+        d.w = _ptr(w)
+        check_squeeze(d, conn, B)
+        return
     if d.kind == _abi.SNN_CONN_SPARSE:
         fill_sparse(d, conn)
         b = getattr(conn, "b", None)
@@ -122,6 +129,10 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
     d.b = _ptr(b) if b is not None else None
     if d.kind == _abi.SNN_CONN_MCC:
         fill_features(d, conn)
+    check_squeeze(d, conn, B)
+
+
+def check_squeeze(d: "_abi.SnnConn", conn, B: int) -> None:
     rule = getattr(conn, "update_rule", None)
     if rule is None and hasattr(conn, "pipeline"):
         rule = conn._weight().learning_rule
@@ -295,11 +306,11 @@ def build_net(
         check_passthrough(net, i, type(conn).__name__)
     conns = [net.conns[i] for i in range(net.n_conns)]
     layers = [net.layers[i] for i in range(net.n_layers)]
-    if (any(d.kind == _abi.SNN_CONN_MAXPOOL2D for d in conns) or any(d.kind in CONVERSION_KINDS for d in layers)) and any(
+    if (any(d.kind in (_abi.SNN_CONN_MAXPOOL2D, _abi.SNN_CONN_LOCAL2D) for d in conns) or any(d.kind in CONVERSION_KINDS for d in layers)) and any(
             d.kind == _abi.SNN_CONN_SPARSE or d.f_prob or d.f_mask or d.f_int for d in conns):
-        raise NotImplementedError("a network with a MaxPool2dConnection, SubtractiveResetIFNodes or PassThroughNodes and a "
-                                  "SparseConnection or MulticompartmentConnection features is not implemented by the CUDA core "
-                                  "(each has its own instantiation of the window kernel)")
+        raise NotImplementedError("a network with a MaxPool2dConnection, LocalConnection2D, SubtractiveResetIFNodes or PassThroughNodes "
+                                  "and a SparseConnection or MulticompartmentConnection features is not implemented by the CUDA "
+                                  "core (each has its own instantiation of the window kernel)")
     return net, keep
 
 

@@ -547,6 +547,99 @@ class MaxPool2dConnection(AbstractConnection):
         d.pool_rates = self.firing_rates.data_ptr()
 
 
+class LocalConnection2D(AbstractConnection):
+    """Two-dimensional locally connected synapses (reference: topology.py:1623-1767): every target neuron has weights of
+    its own over one ``kernel_size`` window of a ``[C, H, W]`` source, ``n_filters`` neurons per window.  ``w`` is
+    ``[in_channels, n_filters * conv_prod, kernel_prod]``; target neuron ``f * conv_prod + p`` sees window ``p``.  Inside
+    ``Network.run`` the generic window kernel gathers each target's receptive field from the source spikes and applies
+    ``PostPre``, ``WeightDependentPostPre``, ``Hebbian`` or ``NoOp``; ``normalize`` scales every ``kernel_prod`` row of
+    ``w`` to sum ``norm``.
+
+    As in the reference: ``w`` is drawn with ``torch.rand`` and clamped when a bound is finite; passing ``w=`` raises
+    ``AttributeError`` (the reference's shape check reads ``self.out_channels``, which it never sets); ``b`` is stored and
+    never used; a target with other than ``n_filters * conv_prod`` neurons raises ``RuntimeError`` when the network runs
+    (the reference's ``view`` fails); ``reset_state_variables`` also resets the target layer.  The rules' update follows
+    the reference's reshape of the unfolded source, which for ``in_channels > 1`` pairs a weight with another source
+    neuron than ``compute`` does (include/snn_b200.h, SNN_CONN_LOCAL2D)."""
+
+    def __init__(self, source: Nodes, target: Nodes, kernel_size, stride, n_filters: int,
+                 nu: Optional[Union[float, Sequence[float], Sequence[torch.Tensor]]] = None, reduction: Optional[callable] = None,
+                 weight_decay: float = 0.0, w_dtype: torch.dtype = torch.float32, **kwargs) -> None:
+        if w_dtype != torch.float32:
+            raise NotImplementedError("bindsnet_b200 computes in float32 only (SURVEY.md §8b)")
+        super().__init__(source, target, nu, reduction, weight_decay, **kwargs)
+        self.kernel_size, self.stride, self.n_filters = _pair(kernel_size), _pair(stride), n_filters
+        self.in_channels, input_height, input_width = source.shape[0], source.shape[1], source.shape[2]
+        height = int((input_height - self.kernel_size[0]) / self.stride[0]) + 1      # topology.py:1677-1682
+        width = int((input_width - self.kernel_size[1]) / self.stride[1]) + 1
+        self.conv_size = (height, width)
+        self.conv_prod = int(np.prod(self.conv_size))
+        self.kernel_prod = int(np.prod(self.kernel_size))
+        if kwargs.get("w", None) is not None:
+            raise AttributeError(f"'{type(self).__name__}' object has no attribute 'out_channels' (the reference's w= shape "
+                                 "check, topology.py:1697-1701, reads an attribute it never sets)")
+        w = torch.rand(self.in_channels, self.n_filters * self.conv_prod, self.kernel_prod)
+        if (self.wmin != -np.inf).any() or (self.wmax != np.inf).any():
+            w = torch.clamp(w, self.wmin, self.wmax)
+        self.w = Parameter(w.contiguous(), requires_grad=False)
+        b = kwargs.get("b", None)
+        self.b = Parameter(torch.as_tensor(b, dtype=torch.float32) if b is not None else torch.empty(0), requires_grad=False)
+
+    def compute(self, s: torch.Tensor) -> torch.Tensor:
+        """topology.py:1717-1740 as the window kernel's receptive-field gather (``snn_b200_conn_compute``)."""
+        from . import _plan
+
+        return _plan.compute_single_connection(self, s)
+
+    def normalize(self) -> None:
+        """topology.py:1748-1759: every row of ``w`` viewed as ``[in_channels * n, kernel_prod]`` scaled to sum ``norm``
+        (a row that sums to zero becomes inf / NaN, as in the reference)."""
+        if self.norm is not None:
+            from . import _plan
+
+            _plan.normalize_single_connection(self)
+
+    def reset_state_variables(self) -> None:
+        """topology.py:1761-1767."""
+        super().reset_state_variables()
+        self.target.reset_state_variables()
+
+    def _check(self) -> None:
+        """The reference's errors at the first ``compute``, raised before anything runs."""
+        if len(self.source.shape) != 3:
+            raise RuntimeError(f"LocalConnection2D needs a [C, H, W] source population, got {list(self.source.shape)}")
+        C_, H, W = (int(v) for v in self.source.shape)
+        if self.kernel_size[0] > H or self.kernel_size[1] > W or min(self.kernel_size) < 1 or min(self.stride) < 1:
+            raise RuntimeError(f"LocalConnection2D: kernel_size {self.kernel_size} / stride {self.stride} do not fit a "
+                               f"{H} x {W} source (unfold fails)")
+        n = self.n_filters * self.conv_prod
+        if self.target.n != n:
+            raise RuntimeError(f"shape '[B, {', '.join(str(int(v)) for v in self.target.shape)}]' is invalid for the "
+                               f"LocalConnection2D output of {n} neurons per sample (n_filters * conv_prod)")
+        if tuple(self.w.shape) != (C_, n, self.kernel_prod):
+            raise RuntimeError(f"LocalConnection2D.w has shape {tuple(self.w.shape)}, expected {(C_, n, self.kernel_prod)}")
+
+    def _fill_desc(self, d: "_abi.SnnConn", dt: float, rule: bool = True) -> None:
+        self._check()
+        d.kind = _abi.SNN_CONN_LOCAL2D
+        if self.wmin.numel() != 1 or self.wmax.numel() != 1:
+            raise NotImplementedError("per-synapse wmin/wmax tensors are not supported by the CUDA core yet")
+        d.wmin = _scalar(self.wmin, "wmin")
+        d.wmax = _scalar(self.wmax, "wmax")
+        d.has_norm = int(self.norm is not None)
+        d.norm_abs = 0
+        d.norm = float(self.norm) if self.norm is not None else 0.0
+        d.dt_scale = 1.0
+        d.cin, d.hin, d.win = (int(v) for v in self.source.shape)
+        d.cout, (d.hout, d.wout) = int(self.n_filters), self.conv_size
+        d.kh, d.kw = self.kernel_size
+        d.sh, d.sw = self.stride
+        d.ph = d.pw = 0
+        d.dh = d.dw = 1
+        if rule:
+            self.update_rule._fill_desc(d)
+
+
 def pool_out_shape(conn):
     """``[C, Hout, Wout]`` of a MaxPool2dConnection (this package's or the reference's: the same attributes), or the
     ``RuntimeError`` the reference's ``compute`` raises for its geometry.  ``F.max_pool2d`` without ceil mode; every window
@@ -621,6 +714,5 @@ Conv3dConnection = _unsupported("Conv3dConnection", "topology.py:847-1025")
 MaxPool1dConnection = _unsupported("MaxPool1dConnection", "topology.py:1028-1121")
 MaxPoo3dConnection = _unsupported("MaxPoo3dConnection", "topology.py:1214-1301")
 LocalConnection1D = _unsupported("LocalConnection1D", "topology.py:1487-1620")
-LocalConnection2D = _unsupported("LocalConnection2D", "topology.py:1623-1767")
 LocalConnection3D = _unsupported("LocalConnection3D", "topology.py:1770-1917")
 MeanFieldConnection = _unsupported("MeanFieldConnection", "topology.py:1920-2006")

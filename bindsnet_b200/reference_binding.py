@@ -9,7 +9,7 @@ a library that implements it — ``libsnn_b200.so`` on CUDA tensors, or the orac
 
 Covered: what ``bindsnet.models`` builds for the hot path — ``Input`` / ``LIFNodes`` / ``DiehlAndCookNodes`` layers,
 ``MulticompartmentConnection`` with one ``Weight`` feature (``MCC_learning.NoOp`` / ``PostPre``) and the classic
-``Connection`` with ``learning.NoOp`` / ``PostPre`` / ``WeightDependentPostPre`` / ``Hebbian``.  Every attribute is read where the
+``Connection`` and ``LocalConnection2D`` with ``learning.NoOp`` / ``PostPre`` / ``WeightDependentPostPre`` / ``Hebbian``.  Every attribute is read where the
 reference keeps it (file:line in the comments); state tensors are handed over by pointer and updated in place.
 """
 from __future__ import annotations
@@ -122,6 +122,34 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
         (d.ph, d.pw), (d.dh, d.dw) = conn.padding, conn.dilation
         d.pool_decay = _f(conn.decay)
         d.pool_rates = fr.data_ptr()
+        return
+    if type(conn).__name__ == "LocalConnection2D":
+        # topology.py:1623-1767: w [in_channels, n_filters * conv_prod, kernel_prod], b never read; the geometry of the
+        # reference's unfold (no padding, no dilation) and its view of the output as the target's shape
+        (d.kh, d.kw), (d.sh, d.sw) = conn.kernel_size, conn.stride
+        d.kind, d.cin, d.hin, d.win = _abi.SNN_CONN_LOCAL2D, *(int(v) for v in conn.source.shape)
+        d.cout, (d.hout, d.wout) = int(conn.n_filters), conn.conv_size
+        d.dh = d.dw = 1
+        if int(conn.target.n) != d.cout * d.hout * d.wout:
+            raise RuntimeError(f"shape '{[B, *conn.target.shape]}' is invalid for the LocalConnection2D output of "
+                               f"{d.cout * d.hout * d.wout} neurons per sample")
+        w = conn.w
+        d.has_norm = int(conn.norm is not None)                                           # topology.py:1748-1759
+        d.norm, d.norm_abs = (_f(conn.norm) if conn.norm is not None else 0.0), 0
+        rule = conn.update_rule
+        name = type(rule).__name__
+        d.rule = {"NoOp": _abi.SNN_RULE_NOOP, "PostPre": _abi.SNN_RULE_POSTPRE, "Hebbian": _abi.SNN_RULE_HEBBIAN,
+                  "WeightDependentPostPre": _abi.SNN_RULE_WDEP_POSTPRE}.get(name, -1)
+        if d.rule < 0:
+            raise NotImplementedError(f"learning rule {name} on a LocalConnection2D")
+        d.nu0, d.nu1 = _f(rule.nu[0]), _f(rule.nu[1])
+        d.reduction = _reduction_code(rule.reduction)
+        d.weight_decay = _f(rule.weight_decay)                                            # learning.py:85
+        d.wmin, d.wmax = _f(conn.wmin), _f(conn.wmax)
+        d.has_clamp = int((math.isfinite(d.wmin) or math.isfinite(d.wmax)) and name != "NoOp")   # learning.py:97-104
+        if w.dtype != torch.float32 or not w.is_contiguous():
+            raise TypeError("weights must be contiguous float32")
+        d.w = w.data_ptr()
         return
     if hasattr(conn, "pipeline"):
         # MulticompartmentConnection (topology.py:402-537) with one Weight feature (topology_features.py:575-671) and at most

@@ -88,6 +88,18 @@ extern "C" {
                                 (step t - 1's, or step t's for an earlier layer in one-step mode), exactly as the
                                 reference's compute(source.s) does.  Generic tier only, and not in a plan that also holds
                                 an SNN_CONN_SPARSE connection or MCC features */
+#define SNN_CONN_LOCAL2D 5 /* LocalConnection2D: per-target (unshared) receptive-field weights, topology.py:1623-1767.
+                              Source [cin,hin,win], target n = cout * P neurons (cout = n_filters, P = hout * wout,
+                              hout = (hin - kh) / sh + 1, wout likewise; ph = pw = 0, dh = dw = 1).  w is [cin, n, K]
+                              with K = kh * kw; b is NULL.  Target n' = f * P + p (p = oy * wout + ox) receives
+                                sum_ci ( sum_k s[ci, oy*sh + k / kw, ox*sw + k % kw] * w[ci, n', k] )
+                              the inner sum over the spiking k ascending from +0, the outer one over ci ascending.
+                              Rules SNN_RULE_NONE / NOOP / POSTPRE / WDEP_POSTPRE / HEBBIAN.  The rules' element
+                              (n', m), m < cin * K, is flat weight n' * cin * K + m, and its source neuron is the one
+                              at flat position (n' % P) * cin * K + m of the unfolded source in [cin, P, K] order (the
+                              reference reshapes that view to [P, cin * K]; for cin = 1 it is the receptive field).
+                              normalize: each row of w viewed as [cin * n, K] scaled by norm / (its sum, ascending k),
+                              no guard against a zero sum.  Generic tier only, not with SNN_CONN_SPARSE or MCC features */
 
 /* ---- learning rules ---- */
 #define SNN_RULE_NONE 0        /* MCC_learning.NoOp: update() does nothing    MCC_learning.py:120-146 */

@@ -97,9 +97,9 @@ struct DevNet {
     int32_t sp_units;             // sparse gather units of a step (0: the plan has no SparseConnection)
     DevSparse sp[SNN_MAX_CONNS];
     int32_t any_feat;             // some MCC connection carries Probability / Mask / Intensity features
-    int32_t any_pool;             // some connection is a MaxPool2dConnection (SNN_CONN_MAXPOOL2D) or a LocalConnection2D
-                                  // (SNN_CONN_LOCAL2D), or some layer is an SNN_NODE_SUBIF / SNN_NODE_PASSTHROUGH one: the
-                                  // plan runs the POOL instantiation
+    int32_t any_pool;             // some connection is a MaxPool2dConnection (SNN_CONN_MAXPOOL2D), a LocalConnection2D
+                                  // (SNN_CONN_LOCAL2D) or a Conv3dConnection (SNN_CONN_CONV3D), or some layer is an
+                                  // SNN_NODE_SUBIF / SNN_NODE_PASSTHROUGH one: the plan runs the POOL instantiation
     float *pool_r1[SNN_MAX_CONNS];   // MaxPool2dConnection: the workspace slot of its rates (pool_rate_slot)
 };
 
@@ -137,6 +137,27 @@ static inline int snn_local2d_geometry_ok(const snn_conn_t &C, int n_src, int n_
     if (C.hout != (C.hin - C.kh) / C.sh + 1 || C.wout != (C.win - C.kw) / C.sw + 1) return SNN_ERR_BAD_ARG;
     if ((long long)C.cin * C.hin * C.win != n_src || (long long)C.cout * C.hout * C.wout != n_tgt) return SNN_ERR_BAD_ARG;
     return SNN_OK;
+}
+
+// A Conv3dConnection's geometry (snn_b200.h): the layer sizes, every output size (in - k + 2p) / s + 1 of a kernel that
+// fits the padded input, no dilation, w and b present.
+static inline int snn_conv3d_out(int in, int k, int s, int p) { return in + 2 * p < k ? 0 : (in - k + 2 * p) / s + 1; }
+static inline int snn_conv3d_geometry_ok(const snn_conn_t &C, int n_src, int n_tgt) {
+    if (!C.w || !C.b) return SNN_ERR_BAD_ARG;
+    if (C.cin < 1 || C.cout < 1 || C.kd < 1 || C.kh < 1 || C.kw < 1 || C.sd < 1 || C.sh < 1 || C.sw < 1) return SNN_ERR_BAD_ARG;
+    if (C.pd < 0 || C.ph < 0 || C.pw < 0 || C.dh != 1 || C.dw != 1) return SNN_ERR_BAD_ARG;
+    if (C.din < 1 || C.hin < 1 || C.win < 1 || C.dout < 1 || C.hout < 1 || C.wout < 1) return SNN_ERR_BAD_ARG;
+    if (C.dout != snn_conv3d_out(C.din, C.kd, C.sd, C.pd) || C.hout != snn_conv3d_out(C.hin, C.kh, C.sh, C.ph) ||
+        C.wout != snn_conv3d_out(C.win, C.kw, C.sw, C.pw))
+        return SNN_ERR_BAD_ARG;
+    if ((long long)C.cin * C.din * C.hin * C.win != n_src || (long long)C.cout * C.dout * C.hout * C.wout != n_tgt) return SNN_ERR_BAD_ARG;
+    return SNN_OK;
+}
+// The updates a Conv3dConnection runs (snn_b200.h): none, learning.NoOp's decay, or a zero-rate PostPre /
+// WeightDependentPostPre (decay and clamp).
+static inline bool snn_conv3d_rule_ok(const snn_conn_t &C) {
+    if (C.rule == SNN_RULE_NONE || C.rule == SNN_RULE_NOOP) return true;
+    return (C.rule == SNN_RULE_POSTPRE || C.rule == SNN_RULE_WDEP_POSTPRE) && C.nu0 == 0.0f && C.nu1 == 0.0f;
 }
 
 __host__ __device__ __forceinline__ int pool_rate_slot(int T, int t) { return (T - 1 - t) & 1; }

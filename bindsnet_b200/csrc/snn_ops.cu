@@ -132,7 +132,39 @@ __global__ void __launch_bounds__(256) pool_compute_kernel(snn_conn_t C, int ns,
     }
 }
 
-__global__ void __launch_bounds__(SNN_GEN_THREADS) conv_normalize_kernel(snn_conn_t C) { normalize_conv_item(C, blockIdx.x, gridDim.x); }
+__global__ void __launch_bounds__(SNN_GEN_THREADS) conv_normalize_kernel(snn_conn_t C, int KK) { normalize_conv_item(C, KK, blockIdx.x, gridDim.x); }
+
+// Conv3dConnection.compute (topology.py:979-995) on byte spikes: the window gather's gather_conv3d order ((ci, kz, ky, kx)
+// ascending from +0, then the bias).  Thread = one target neuron of one sample.
+__global__ void __launch_bounds__(256) conv3d_compute_kernel(snn_conn_t C, int ns, int nt, int B, const uint8_t *__restrict__ s,
+                                                             float *__restrict__ out) {
+    const size_t total = (size_t)B * nt;
+    const int HW = C.hout * C.wout, L = C.dout * HW, KK = C.kd * C.kh * C.kw;
+    for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+        const int b = (int)(e / nt), j = (int)(e - (size_t)b * nt), co = j / L, l = j - co * L;
+        const int oz = l / HW, r = l - oz * HW, oy = r / C.wout, ox = r - oy * C.wout;
+        const uint8_t *sb = s + (size_t)b * ns;
+        const float *wf = C.w + (size_t)co * C.cin * KK;
+        float p = 0.0f;
+        for (int ci = 0; ci < C.cin; ++ci)
+            for (int kz = 0; kz < C.kd; ++kz) {
+                const int iz = oz * C.sd - C.pd + kz;
+                if (iz < 0 || iz >= C.din) continue;
+                for (int ky = 0; ky < C.kh; ++ky) {
+                    const int iy = oy * C.sh - C.ph + ky;
+                    if (iy < 0 || iy >= C.hin) continue;
+                    for (int kx = 0; kx < C.kw; ++kx) {
+                        const int ix = ox * C.sw - C.pw + kx;
+                        if (ix < 0 || ix >= C.win) continue;
+                        if (sb[((ci * C.din + iz) * C.hin + iy) * C.win + ix]) p = p + wf[((ci * C.kd + kz) * C.kh + ky) * C.kw + kx];
+                    }
+                }
+            }
+        out[e] = p + C.b[co];
+    }
+}
+
+__global__ void __launch_bounds__(SNN_GEN_THREADS) conv3d_update_kernel(snn_conn_t C) { phase3_conv3d(C, blockIdx.x, gridDim.x); }
 
 // LocalConnection2D.compute (topology.py:1717-1740) on byte spikes: the window gather's gather_local2d order (k ascending
 // within a channel from +0, then the channels).  Thread = one target neuron of one sample.
@@ -263,6 +295,14 @@ int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, 
         SNN_LAUNCH(local2d_compute_kernel, blocks, 256, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
         return cuda_rc(cudaGetLastError());
     }
+    if (conn->kind == SNN_CONN_CONV3D) {
+        const int rc = snn_conv3d_geometry_ok(*conn, n_src, n_tgt);
+        if (rc != SNN_OK) return rc;
+        const size_t total = (size_t)B * n_tgt;
+        const int blocks = (int)((total + 255) / 256 < 4736 ? (total + 255) / 256 : 4736);
+        SNN_LAUNCH(conv3d_compute_kernel, blocks, 256, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
+        return cuda_rc(cudaGetLastError());
+    }
     if (conn->kind == SNN_CONN_CONV2D) {
         if (!conn->b || conn->cin * conn->hin * conn->win != n_src || conn->cout * conn->hout * conn->wout != n_tgt) return SNN_ERR_BAD_ARG;
         const size_t total = (size_t)B * n_tgt;
@@ -298,6 +338,16 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
         return cuda_rc(cudaGetLastError());
     }
     if (!C.w) return SNN_ERR_BAD_ARG;
+    if (C.kind == SNN_CONN_CONV3D) {   // decay / clamp only (snn_b200.h), dense over w
+        const int rc = snn_conv3d_geometry_ok(C, net->layers[C.src].n, net->layers[C.tgt].n);
+        if (rc != SNN_OK) return rc;
+        if (!snn_conv3d_rule_ok(C) || C.mask) return SNN_ERR_UNSUPPORTED;
+        if (C.rule == SNN_RULE_NONE) return SNN_OK;
+        const size_t NW = (size_t)C.cout * C.cin * C.kd * C.kh * C.kw;
+        const int blocks = (int)((NW + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS < 1184 ? (NW + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS : 1184);
+        SNN_LAUNCH(conv3d_update_kernel, blocks, SNN_GEN_THREADS, 0, (cudaStream_t)stream_, C);
+        return cuda_rc(cudaGetLastError());
+    }
     const bool pass = net->layers[C.src].kind == SNN_NODE_PASSTHROUGH || net->layers[C.tgt].kind == SNN_NODE_PASSTHROUGH;
     if (pass && C.rule != SNN_RULE_NONE && C.rule != SNN_RULE_NOOP) return SNN_ERR_UNSUPPORTED;   // (snn_b200.h)
     // the single-operator update is the dense [n_src, n_tgt] rule application or a LocalConnection2D's; convolutional
@@ -356,7 +406,13 @@ int snn_b200_conn_normalize(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt
     }
     if (conn->kind == SNN_CONN_CONV2D) {
         const int F = conn->cout * conn->cin;
-        SNN_LAUNCH(conv_normalize_kernel, (F + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn);
+        SNN_LAUNCH(conv_normalize_kernel, (F + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, conn->kh * conn->kw);
+        return cuda_rc(cudaGetLastError());
+    }
+    if (conn->kind == SNN_CONN_CONV3D) {   // rows of w viewed as [cout * cin, kd * kh * kw]
+        const int F = conn->cout * conn->cin;
+        SNN_LAUNCH(conv_normalize_kernel, (F + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn,
+                   conn->kd * conn->kh * conn->kw);
         return cuda_rc(cudaGetLastError());
     }
     SNN_LAUNCH(conn_normalize_kernel, (n_tgt + SNN_TILE - 1) / SNN_TILE, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, n_src, n_tgt);

@@ -373,6 +373,43 @@ __device__ __forceinline__ float gather_conv(const snn_conn_t &C, const uint32_t
     return p + C.b[co];
 }
 
+// Conv3dConnection.compute (topology.py:979-995) for one target neuron j = (co, oz, oy, ox) of one sample: the sum of the
+// filter taps whose (zero-padded) input position spiked, in ascending (ci, kz, ky, kx) order from +0, then the bias
+// (gather_conv's order with a depth loop).  The valid taps of a kernel row look at consecutive source bits: each run of
+// up to 32 is cut out of the bit row with one funnel shift and only its set bits are visited.  STAGED_BITS / STAGED_TAPS:
+// the sample's source bit row / the taps of the tile's output channels sit in shared memory (staged by phase 1).
+template <bool STAGED_BITS, bool STAGED_TAPS>
+__device__ __forceinline__ float gather_conv3d(const snn_conn_t &C, const uint32_t *sb, const float *taps, int co_base, int j, bool valid) {
+    if (!valid) return 0.0f;
+    const int HW = C.hout * C.wout, L = C.dout * HW, co = j / L, l = j - co * L;
+    const int oz = l / HW, r = l - oz * HW, oy = r / C.wout, ox = r - oy * C.wout;
+    const int iz0 = oz * C.sd - C.pd, iy0 = oy * C.sh - C.ph, ix0 = ox * C.sw - C.pw;
+    const int kz_lo = max(0, -iz0), kz_hi = min(C.kd, C.din - iz0);
+    const int ky_lo = max(0, -iy0), ky_hi = min(C.kh, C.hin - iy0);
+    const int kx_lo = max(0, -ix0), kx_hi = min(C.kw, C.win - ix0);
+    const int KK = C.kd * C.kh * C.kw;
+    const float *tp = STAGED_TAPS ? taps + (size_t)(co - co_base) * C.cin * KK : C.w + (size_t)co * C.cin * KK;
+    float p = 0.0f;
+    for (int ci = 0; ci < C.cin; ++ci)
+        for (int kz = kz_lo; kz < kz_hi; ++kz)
+            for (int ky = ky_lo; ky < ky_hi; ++ky) {
+                const int row = ((ci * C.din + iz0 + kz) * C.hin + iy0 + ky) * C.win + ix0;   // source bit of tap kx = 0
+                const int k0 = ((ci * C.kd + kz) * C.kh + ky) * C.kw;
+                for (int kx = kx_lo; kx < kx_hi; kx += 32) {
+                    const int cnt = min(32, kx_hi - kx), bit0 = row + kx, w0 = bit0 >> 5, sft = bit0 & 31;
+                    const uint32_t lo = STAGED_BITS ? sb[w0] : __ldcg(sb + w0);
+                    const uint32_t hi = sft + cnt > 32 ? (STAGED_BITS ? sb[w0 + 1] : __ldcg(sb + w0 + 1)) : 0u;
+                    uint32_t bits = __funnelshift_r(lo, hi, sft) & (cnt >= 32 ? 0xffffffffu : ((1u << cnt) - 1u));
+                    while (bits) {
+                        const int k = k0 + kx + __ffs(bits) - 1;
+                        bits &= bits - 1;
+                        p = p + (STAGED_TAPS ? tp[k] : __ldcg(tp + k));
+                    }
+                }
+            }
+    return p + C.b[co];
+}
+
 // LocalConnection2D.compute (topology.py:1717-1740) for target neuron j = (f, oy, ox) of one sample (n target neurons):
 // per input channel the sum of its own weights w[ci, j, k] whose window position k spiked (k ascending, from +0), then
 // the channel sums in ascending ci (the reference's sum(-1).sum(1)).  The kw window bits of a kernel row are cut out of
@@ -549,12 +586,15 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
     int cnt = 0;  // candidates of this column over this warp's samples
 
     // a convolutional input: stage the chunk's source bit rows and the taps of this tile's output channels (POOL: a
-    // LocalConnection2D input gets its bit rows staged the same way; its weights are per target, not taps)
+    // Conv3dConnection input likewise, with the depth axis in its channel size and taps; a LocalConnection2D input gets
+    // its bit rows staged the same way, its weights are per target, not taps)
     int conv_c = -1, conv_slot = 0, co_base = 0;
     bool st_bits = false, st_taps = false;
     ConvGeo geo = {};
     for (int c = 0; c < N.n_conns && conv_c < 0; ++c)
-        if (N.conns[c].tgt == li && (N.conns[c].kind == SNN_CONN_CONV2D || (POOL && N.conns[c].kind == SNN_CONN_LOCAL2D))) conv_c = c;
+        if (N.conns[c].tgt == li &&
+            (N.conns[c].kind == SNN_CONN_CONV2D || (POOL && (N.conns[c].kind == SNN_CONN_LOCAL2D || N.conns[c].kind == SNN_CONN_CONV3D))))
+            conv_c = c;
     if (conv_c >= 0) {
         const snn_conn_t &C = N.conns[conv_c];
         const DevLayer &S = N.layers[C.src];
@@ -562,11 +602,12 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
         conv_slot = (N.one_step && C.src < li) ? wr : rd;
         const int words = (b1 - b0) * S.nw;
         st_bits = words <= SNN_CONV_STAGE_WORDS;
-        const int Lhw = C.hout * C.wout, K = C.cin * C.kh * C.kw;
+        const bool c3 = POOL && C.kind == SNN_CONN_CONV3D;
+        const int Lhw = C.hout * C.wout * (c3 ? C.dout : 1), K = C.cin * C.kh * C.kw * (c3 ? C.kd : 1);
         co_base = (tile * SNN_TILE) / Lhw;
         const int co_hi = min(n - 1, tile * SNN_TILE + SNN_TILE - 1) / Lhw;
         const int ntaps = (co_hi - co_base + 1) * K;
-        st_taps = ntaps <= SNN_CONV_STAGE_TAPS && (!POOL || C.kind == SNN_CONN_CONV2D);
+        st_taps = ntaps <= SNN_CONV_STAGE_TAPS && (!POOL || C.kind != SNN_CONN_LOCAL2D);
         if (st_bits) {
             const uint32_t *src = S.bits + ((size_t)conv_slot * B + b0) * S.nw;
             for (int k0 = threadIdx.x; k0 < words; k0 += 4 * SNN_GEN_THREADS) {
@@ -602,7 +643,8 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
         for (int q = 0; q < 4; ++q) {
             fwn[q] = 0u; afn[q] = 1u;
             if (q < ncl && b < b1 && N.conns[cl[q]].kind != SNN_CONN_CONV2D && !(SPARSE && N.conns[cl[q]].kind == SNN_CONN_SPARSE) &&
-                !(POOL && (N.conns[cl[q]].kind == SNN_CONN_MAXPOOL2D || N.conns[cl[q]].kind == SNN_CONN_LOCAL2D))) {
+                !(POOL && (N.conns[cl[q]].kind == SNN_CONN_MAXPOOL2D || N.conns[cl[q]].kind == SNN_CONN_LOCAL2D ||
+                           N.conns[cl[q]].kind == SNN_CONN_CONV3D))) {
                 const snn_conn_t &C = N.conns[cl[q]];
                 const DevLayer &S = N.layers[C.src];
                 const int slot = (N.one_step && C.src < li) ? wr : rd;
@@ -659,6 +701,16 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
                 const uint32_t *sb = S.bits + ((size_t)slot * B + b) * S.nw;
                 const int i = valid ? pool_argmax(C, r, j) : 0;
                 p = (valid && ((__ldcg(sb + (i >> 5)) >> (i & 31)) & 1u)) ? 1.0f : 0.0f;
+            } else if (POOL && C.kind == SNN_CONN_CONV3D) {
+                const uint32_t *gsb = S.bits + ((size_t)slot * B + b) * S.nw;
+                if (c == conv_c && st_bits) {
+                    const uint32_t *ssb = M.cbits + (size_t)(b - b0) * S.nw;
+                    p = st_taps ? gather_conv3d<true, true>(C, ssb, M.xs, co_base, j, valid) : gather_conv3d<true, false>(C, ssb, nullptr, 0, j, valid);
+                } else if (c == conv_c && st_taps) {
+                    p = gather_conv3d<false, true>(C, gsb, M.xs, co_base, j, valid);
+                } else {
+                    p = gather_conv3d<false, false>(C, gsb, nullptr, 0, j, valid);
+                }
             } else if (POOL && C.kind == SNN_CONN_LOCAL2D) {
                 p = c == conv_c && st_bits ? gather_local2d<true>(C, M.cbits + (size_t)(b - b0) * S.nw, n, j, valid)
                                            : gather_local2d<false>(C, S.bits + ((size_t)slot * B + b) * S.nw, n, j, valid);
@@ -1261,6 +1313,22 @@ __device__ void phase3_local2d(const DevNet &N, int ci_, int cta, int ncta, int 
     }
 }
 
+// The updates a Conv3dConnection runs (snn_b200.h, snn_conv3d_rule_ok): learning.NoOp's w *= weight_decay
+// (learning.py:93-94), and a zero-rate PostPre / WeightDependentPostPre's decay then clamp (:87-104).  Dense over w and
+// spread over the grid (cta of ncta), like the conv2d NoOp branch.
+__device__ void phase3_conv3d(const snn_conn_t &C, int cta, int ncta) {
+    const size_t NW = (size_t)C.cout * C.cin * C.kd * C.kh * C.kw;
+    const size_t start = (size_t)cta * SNN_GEN_THREADS + threadIdx.x, stride = (size_t)ncta * SNN_GEN_THREADS;
+    const bool clamp = C.rule != SNN_RULE_NOOP && C.has_clamp;
+    if (C.weight_decay == 0.0f && !clamp) return;
+    for (size_t e = start; e < NW; e += stride) {
+        float x = __ldcg(C.w + e);
+        if (C.weight_decay != 0.0f) x = x * C.weight_decay;
+        if (clamp) x = clampf(x, C.wmin, C.wmax);
+        C.w[e] = x;
+    }
+}
+
 // learning.MSTDP._conv2d_connection_update (learning.py:1942-2015) with a per-sample eligibility
 // (SURVEY.md §0.8), PostPre / WeightDependentPostPre / Hebbian on a Conv2dConnection, and the decay-only
 // update of a conv connection without a rule (learning.NoOp).  Called once per CTA and step: every loop is
@@ -1534,8 +1602,10 @@ __device__ __forceinline__ void decay_sparse(const snn_conn_t &C, int cta, int n
 
 // Conv2dConnection.normalize (topology.py:824-837): every (out, in) filter scaled to sum `norm`
 // (plain sum in ascending order; no guard against a zero sum, like the reference).
-__device__ void normalize_conv_item(const snn_conn_t &C, int tile, int ntiles) {
-    const int F = C.cout * C.cin, KK = C.kh * C.kw;
+// Conv2dConnection.normalize (topology.py:824-837) and Conv3dConnection.normalize (:1004-1018): every (out, in) filter of
+// KK taps (kh * kw, or kd * kh * kw) scaled by norm / its sum.
+__device__ void normalize_conv_item(const snn_conn_t &C, int KK, int tile, int ntiles) {
+    const int F = C.cout * C.cin;
     for (int f = tile * SNN_GEN_THREADS + threadIdx.x; f < F; f += ntiles * SNN_GEN_THREADS) {
         float tot = 0.0f;
         for (int k = 0; k < KK; ++k) tot = tot + C.w[(size_t)f * KK + k];

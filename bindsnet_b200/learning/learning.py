@@ -1,7 +1,8 @@
 """Learning rules for ``Connection`` — host-side mirror of ``bindsnet/learning/learning.py``
 (``LearningRule`` :25-104, ``NoOp`` :107-146, ``PostPre`` :149-420 / :457-497 (conv2d),
 ``WeightDependentPostPre`` :562-653 / :920-975, ``Hebbian`` :1052-1136 / :1348-1380, ``MSTDP``; the three unsupervised
-rules also on ``LocalConnection2D``, :258-320 / :717-791 / :1186-1250).  The rule objects hold hyper-parameters; the update
+rules also on ``LocalConnection2D``, :258-320 / :717-791 / :1186-1250; on ``Conv3dConnection`` only what the reference
+can run, see ``Conv3dConnection``).  The rule objects hold hyper-parameters; the update
 itself is fused into the CUDA window kernels (``Network.run``) or submitted for one step by
 ``rule.update()``."""
 from __future__ import annotations
@@ -96,11 +97,17 @@ class LearningRule(ABC):
 def _check_connection(rule, connection) -> None:
     """The STDP-family rules exist for ``Connection`` (``_connection_update``), ``Conv2dConnection``
     (``_conv2d_connection_update``) and ``LocalConnection2D`` (``_local_connection2d_update``); the reference's im2col
-    ignores dilation, so a dilated filter is refused."""
-    from ..network.topology import Connection, Conv2dConnection, LocalConnection2D
+    ignores dilation, so a dilated filter is refused.  On ``Conv3dConnection`` (``_conv3d_connection_update``) the
+    post-synaptic-only form of PostPre / WeightDependentPostPre pairs the kernel axes transposed against ``w``
+    (learning.py:517-530, 996-1010); it is not built, so such a rule is refused here."""
+    from ..network.topology import Connection, Conv2dConnection, Conv3dConnection, LocalConnection2D
 
-    if not isinstance(connection, (Connection, Conv2dConnection, LocalConnection2D)):
+    if not isinstance(connection, (Connection, Conv2dConnection, LocalConnection2D, Conv3dConnection)):
         raise NotImplementedError("This learning rule is not supported for this Connection type.")
+    if isinstance(connection, Conv3dConnection) and isinstance(rule, (PostPre, WeightDependentPostPre)) and \
+            float(rule.nu[0]) == 0.0 and float(rule.nu[1]) != 0.0:
+        raise NotImplementedError(f"{type(rule).__name__} with only a post-synaptic rate on a Conv3dConnection: the reference "
+                                  "pairs its kernel axes transposed against w, which is not implemented (DESIGN.md section 8)")
     if isinstance(connection, Conv2dConnection) and connection._geometry[3] != (1, 1):
         raise NotImplementedError(f"{type(rule).__name__} on a dilated Conv2dConnection is undefined in the reference (im2col ignores dilation)")
 
@@ -168,11 +175,13 @@ class MSTDP(_RewardModulated, LearningRule):
 
     def __init__(self, connection, nu=None, reduction=None, weight_decay: float = 0.0, **kwargs) -> None:
         super().__init__(connection=connection, nu=nu, reduction=reduction, weight_decay=weight_decay, **kwargs)
-        from ..network.topology import Connection, Conv2dConnection
+        from ..network.topology import Connection, Conv2dConnection, Conv3dConnection
 
-        if not isinstance(connection, (Connection, Conv2dConnection)):
+        if not isinstance(connection, (Connection, Conv2dConnection, Conv3dConnection)):
             raise NotImplementedError("This learning rule is not supported for this Connection type.")
         self._conv = isinstance(connection, Conv2dConnection)
+        # built as in the reference; its learning windows are refused (Conv3dConnection._check_learning)
+        self._conv3d = isinstance(connection, Conv3dConnection)
         if self._conv and connection._geometry[3] != (1, 1):
             raise NotImplementedError("MSTDP on a dilated Conv2dConnection is undefined in the reference (im2col ignores dilation)")
         self.tc_plus = torch.tensor(kwargs.get("tc_plus", 20.0))
@@ -184,6 +193,8 @@ class MSTDP(_RewardModulated, LearningRule):
 
     def _prepare(self, B: int, dev: torch.device, run_kwargs: dict) -> None:
         """Allocate / validate the rule state for a window (learning.py:1519-1535, 1958-1961, 1979-1991)."""
+        if self._conv3d:   # the rule never runs (Conv3dConnection._check_learning): no state
+            return
         self._take_run_kwargs(run_kwargs)
         src, tgt = self.source, self.target
         if self._conv:
@@ -223,6 +234,8 @@ class MSTDPET(_EligibilityTrace, MSTDP):
         self.tc_e_trace = torch.tensor(kwargs.get("tc_e_trace", 25.0))
 
     def _prepare(self, B: int, dev: torch.device, run_kwargs: dict) -> None:
+        if self._conv3d:
+            return
         self._prepare_trace(B, tuple(self.connection.w.shape), dev)
         super()._prepare(B, dev, run_kwargs)
 

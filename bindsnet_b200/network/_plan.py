@@ -106,6 +106,12 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
         d.w = _ptr(w)
         check_squeeze(d, conn, B)
         return
+    if d.kind == _abi.SNN_CONN_CONV3D:   # [cout, cin, kd, kh, kw] weights and [cout] bias (shapes checked by _fill_desc)
+        w, b = conn.w, conn.b
+        if w.dtype != torch.float32 or not w.is_contiguous() or b.dtype != torch.float32 or not b.is_contiguous():
+            raise TypeError("connection weights and bias must be contiguous float32")
+        d.w, d.b = _ptr(w), _ptr(b)
+        return   # (no batch reduction runs: its rules are decay and clamp only)
     if d.kind == _abi.SNN_CONN_SPARSE:
         fill_sparse(d, conn)
         b = getattr(conn, "b", None)
@@ -306,11 +312,12 @@ def build_net(
         check_passthrough(net, i, type(conn).__name__)
     conns = [net.conns[i] for i in range(net.n_conns)]
     layers = [net.layers[i] for i in range(net.n_layers)]
-    if (any(d.kind in (_abi.SNN_CONN_MAXPOOL2D, _abi.SNN_CONN_LOCAL2D) for d in conns) or any(d.kind in CONVERSION_KINDS for d in layers)) and any(
+    pool_kinds = (_abi.SNN_CONN_MAXPOOL2D, _abi.SNN_CONN_LOCAL2D, _abi.SNN_CONN_CONV3D)
+    if (any(d.kind in pool_kinds for d in conns) or any(d.kind in CONVERSION_KINDS for d in layers)) and any(
             d.kind == _abi.SNN_CONN_SPARSE or d.f_prob or d.f_mask or d.f_int for d in conns):
-        raise NotImplementedError("a network with a MaxPool2dConnection, LocalConnection2D, SubtractiveResetIFNodes or PassThroughNodes "
-                                  "and a SparseConnection or MulticompartmentConnection features is not implemented by the CUDA "
-                                  "core (each has its own instantiation of the window kernel)")
+        raise NotImplementedError("a network with a MaxPool2dConnection, LocalConnection2D, Conv3dConnection, SubtractiveResetIFNodes or "
+                                  "PassThroughNodes and a SparseConnection or MulticompartmentConnection features is not "
+                                  "implemented by the CUDA core (each has its own instantiation of the window kernel)")
     return net, keep
 
 
@@ -410,6 +417,8 @@ def _fill_endpoint(d: "_abi.SnnLayer", layer, name: str, B: int) -> None:
 def update_single_connection(conn) -> None:
     """``conn.update(learning=True)`` from the layers' current ``s`` / ``x``."""
     B = conn.source.s.shape[0]
+    if hasattr(conn, "_check_learning"):   # (Conv3dConnection: the rules the reference cannot run)
+        conn._check_learning()
     _backend.require_cuda(conn.w, "connection weights")
     net = _pair_net(conn, B)
     _backend.conn_update(net, 0, B, conn.w.device)

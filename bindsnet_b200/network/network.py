@@ -253,6 +253,9 @@ class Network(torch.nn.Module):
                 for c in self.connections.values():
                     c.normalize()
             return
+        for conn in self.connections.values():   # errors the reference raises inside the window, before anything runs
+            if hasattr(conn, "_check_window"):
+                conn._check_window(bool(self.learning))
         ext = {k: self._stage_input(k, v, T, dev) for k, v in inputs.items() if k in self.layers}
         clamps = {k: self._stage_mask(k, v, T, dev, False) for k, v in (clamp or {}).items() if v is not None}
         unclamps = {k: self._stage_mask(k, v, T, dev, False) for k, v in (unclamp or {}).items() if v is not None}
@@ -378,7 +381,7 @@ class Network(torch.nn.Module):
             if type(layer) not in builtin_nodes and (layer.kind is None or type(layer).forward is not N.Nodes.forward):
                 return True
         builtin_conns = (Tp.Connection, Tp.MulticompartmentConnection, Tp.Conv2dConnection, Tp.LocalConnection, Tp.SparseConnection,
-                         Tp.MaxPool2dConnection, Tp.LocalConnection2D)
+                         Tp.MaxPool2dConnection, Tp.LocalConnection2D, Tp.Conv3dConnection)
         for conn in self.connections.values():
             if type(conn) not in builtin_conns:
                 return True

@@ -237,6 +237,154 @@ class Conv2dConnection(AbstractConnection):
             self.update_rule._fill_desc(d)
 
 
+def _triple(x):
+    return tuple(x) if isinstance(x, (tuple, list)) else (x, x, x)
+
+
+class Conv3dConnection(AbstractConnection):
+    """3-D convolutional synapses (reference: topology.py:847-1025).  Source and target populations are
+    ``[C, D, H, W]`` shaped; ``w`` is ``[out_channels, in_channels, kd, kh, kw]``, ``b`` ``[out_channels]`` (zeros by
+    default).  Inside ``Network.run`` the convolution is a spike-gather over each target neuron's receptive field;
+    ``normalize`` scales every ``(out, in)`` filter to sum ``norm``.
+
+    As in the reference: a dilation other than 1 raises ``NotImplementedError``; a target whose shape is not
+    ``[out_channels, D', H', W']`` with each size ``int((in - k + 2p) / s + 1)`` raises ``AssertionError``; ``w`` is drawn
+    with ``torch.rand`` and clamped or scaled like ``Conv2dConnection``'s.  The reference's learning rules on this class
+    multiply the bool source spikes by a float trace, which fails; so a learning window whose rule evaluates that
+    pre-synaptic term (``PostPre`` / ``WeightDependentPostPre`` with ``nu[0] != 0``, ``Hebbian``, ``MSTDP``, ``MSTDPET``)
+    raises the reference's ``RuntimeError`` before it starts.  ``NoOp`` decays ``w``; ``PostPre`` /
+    ``WeightDependentPostPre`` with both rates zero decay and clamp it.  Their post-synaptic-only form pairs the kernel
+    axes transposed against ``w`` (learning.py:517-530) and is refused when the rule is built (DESIGN.md section 8)."""
+
+    def __init__(
+        self,
+        source: Nodes,
+        target: Nodes,
+        kernel_size,
+        stride=1,
+        padding=0,
+        dilation=1,
+        nu: Optional[Union[float, Sequence[float], Sequence[torch.Tensor]]] = None,
+        reduction: Optional[callable] = None,
+        weight_decay: float = 0.0,
+        w_dtype: torch.dtype = torch.float32,
+        **kwargs,
+    ) -> None:
+        if w_dtype != torch.float32:
+            raise NotImplementedError("bindsnet_b200 computes in float32 only (SURVEY.md §8b)")
+        super().__init__(source, target, nu, reduction, weight_decay, **kwargs)
+        if dilation != 1 and dilation != (1, 1, 1):                                       # topology.py:899-903
+            raise NotImplementedError("Dilation is not currently supported for 3-D spiking convolution.")
+        self.kernel_size, self.stride = _triple(kernel_size), _triple(stride)
+        self.padding, self.dilation = _triple(padding), _triple(dilation)
+        self.in_channels, input_depth, input_height, input_width = (source.shape[0], source.shape[1], source.shape[2], source.shape[3])
+        self.out_channels = target.shape[0]
+        # topology.py:922-952 (the reference swaps the names width / height; the values are these)
+        out = [int((i - k + 2 * p) / s + 1) for i, k, p, s in
+               zip((input_depth, input_height, input_width), self.kernel_size, self.padding, self.stride)]
+        assert target.shape[1] == out[0] and target.shape[2] == out[1] and target.shape[3] == out[2], (
+            "Target dimensionality must be (out_channels, ?,"
+            "(input_depth - filter_depth + 2 * padding_depth) / stride_depth + 1,"
+            "(input_height - filter_height + 2 * padding_height) / stride_height + 1,"
+            "(input_width - filter_width + 2 * padding_width) / stride_width + 1"
+        )
+        w = kwargs.get("w", None)
+        shape = (self.out_channels, self.in_channels, *self.kernel_size)
+        if w is None:
+            # topology.py:954-968
+            if (self.wmin == -np.inf).any() or (self.wmax == np.inf).any():
+                w = torch.clamp(torch.rand(*shape), self.wmin, self.wmax)
+            else:
+                w = (self.wmax - self.wmin) * torch.rand(*shape)
+                w = w + self.wmin
+        else:
+            # topology.py:969-972
+            w = torch.as_tensor(w)
+            if (self.wmin == -np.inf).any() or (self.wmax == np.inf).any():
+                w = torch.clamp(w, self.wmin, self.wmax)
+            w = self.cast_dtype_if_needed(w, w_dtype)
+        self.w = Parameter(w.detach().clone().float().contiguous(), requires_grad=False)
+        self.b = Parameter(torch.as_tensor(kwargs.get("b", torch.zeros(self.out_channels)), dtype=torch.float32).clone(),
+                           requires_grad=False)
+
+    def compute(self, s: torch.Tensor) -> torch.Tensor:
+        """``F.conv3d(s.float(), w, b, stride, padding)`` for {0,1} spikes (topology.py:979-995), as the spike-gather the
+        window kernel uses (``snn_b200_conn_compute``)."""
+        from . import _plan
+
+        return _plan.compute_single_connection(self, s)
+
+    def normalize(self) -> None:
+        """Every (out, in) filter scaled to sum ``norm`` (topology.py:1004-1018; a filter that sums to zero becomes
+        inf / NaN, as in the reference); also runs at the end of every ``Network.run`` window."""
+        if self.norm is not None:
+            from . import _plan
+
+            _plan.normalize_single_connection(self)
+
+    def _check(self) -> None:
+        """The errors of the reference's first ``compute`` (F.conv3d), raised before anything runs."""
+        if any(int(v) == 0 for v in self.target.shape):
+            k = "x".join(str(v) for v in self.kernel_size)
+            raise RuntimeError(f"Conv3dConnection: calculated output size {list(self.target.shape)} is too small (kernel {k}, "
+                               f"padded input {[int(v) + 2 * p for v, p in zip(self.source.shape[1:], self.padding)]})")
+        shape = (int(self.out_channels), int(self.in_channels), *self.kernel_size)
+        if tuple(self.w.shape) != shape:
+            raise RuntimeError(f"Conv3dConnection.w has shape {tuple(self.w.shape)}, expected {shape}")
+        if tuple(self.b.shape) != (shape[0],):
+            raise RuntimeError(f"Given weight of size {list(self.w.shape)}, expected bias to be 1-dimensional with {shape[0]} "
+                               f"elements, but got bias of size {list(self.b.shape)} instead")
+
+    def _check_learning(self) -> None:
+        """The reference's update on this class (learning.py:499-559, 978-1050, 1382-1438, 2017-2121, 2739-2855) fails
+        in ``torch.bmm`` whenever it evaluates the pre-synaptic term: the unfolded source spikes stay bool.  Raised when
+        a learning window or a standalone update would run it, before any state changes."""
+        from ..learning import learning as L
+
+        rule = self.update_rule
+        pre = isinstance(rule, (L.Hebbian, L.MSTDP)) or (
+            isinstance(rule, (L.PostPre, L.WeightDependentPostPre)) and bool(rule.nu[0] != 0))
+        if pre:
+            raise RuntimeError("expected m1 and m2 to have the same dtype, but got: float != bool (the reference's "
+                               f"{type(rule).__name__} on a Conv3dConnection multiplies the bool source spikes)")
+        if isinstance(rule, (L.PostPre, L.WeightDependentPostPre)):
+            # the unfolds it runs even at zero rates pair depth with kw, height with kh, width with kd (learning.py:517-545)
+            (D, H, W), (p0, p1, p2) = (int(v) for v in self.source.shape[1:]), self.padding
+            kd, kh, kw = self.kernel_size
+            if D + 2 * p2 < kw or H + 2 * p1 < kh or W + 2 * p0 < kd:
+                raise RuntimeError(f"maximum size for tensor at an unfolded dimension is smaller than the kernel: the "
+                                   f"reference's {type(rule).__name__} update on this Conv3dConnection fails")
+
+    def _check_window(self, learning: bool) -> None:
+        self._check()
+        if learning:
+            self._check_learning()
+
+    def _fill_desc(self, d: "_abi.SnnConn", dt: float, rule: bool = True) -> None:
+        from ..learning import learning as L
+
+        self._check()
+        d.kind = _abi.SNN_CONN_CONV3D
+        if self.wmin.numel() != 1 or self.wmax.numel() != 1:
+            raise NotImplementedError("per-synapse wmin/wmax tensors are not supported by the CUDA core yet")
+        d.wmin = _scalar(self.wmin, "wmin")
+        d.wmax = _scalar(self.wmax, "wmax")
+        d.has_norm = int(self.norm is not None)
+        d.norm_abs = 0
+        d.norm = float(self.norm) if self.norm is not None else 0.0
+        d.dt_scale = 1.0
+        d.cin, d.din, d.hin, d.win = (int(v) for v in self.source.shape)
+        d.cout, d.dout, d.hout, d.wout = (int(v) for v in self.target.shape)
+        d.kd, d.kh, d.kw = self.kernel_size
+        d.sd, d.sh, d.sw = self.stride
+        d.pd, d.ph, d.pw = self.padding
+        d.dh = d.dw = 1
+        # a rule that evaluates the pre-synaptic term never runs (_check_learning refuses its learning windows): the plan
+        # of a window without learning carries no rule for it
+        if rule and type(self.update_rule) in (L.NoOp, L.PostPre, L.WeightDependentPostPre):
+            self.update_rule._fill_desc(d)
+
+
 class AbstractMulticompartmentConnection(ABC, Module):
     """Reference: topology.py:159-262."""
 
@@ -710,7 +858,6 @@ def _unsupported(name: str, where: str):
 
 
 Conv1dConnection = _unsupported("Conv1dConnection", "topology.py:540-683")
-Conv3dConnection = _unsupported("Conv3dConnection", "topology.py:847-1025")
 MaxPool1dConnection = _unsupported("MaxPool1dConnection", "topology.py:1028-1121")
 MaxPoo3dConnection = _unsupported("MaxPoo3dConnection", "topology.py:1214-1301")
 LocalConnection1D = _unsupported("LocalConnection1D", "topology.py:1487-1620")

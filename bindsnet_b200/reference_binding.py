@@ -9,7 +9,8 @@ a library that implements it — ``libsnn_b200.so`` on CUDA tensors, or the orac
 
 Covered: what ``bindsnet.models`` builds for the hot path — ``Input`` / ``LIFNodes`` / ``DiehlAndCookNodes`` layers,
 ``MulticompartmentConnection`` with one ``Weight`` feature (``MCC_learning.NoOp`` / ``PostPre``) and the classic
-``Connection`` and ``LocalConnection2D`` with ``learning.NoOp`` / ``PostPre`` / ``WeightDependentPostPre`` / ``Hebbian``.  Every attribute is read where the
+``Connection`` and ``LocalConnection2D`` with ``learning.NoOp`` / ``PostPre`` / ``WeightDependentPostPre`` / ``Hebbian``,
+``Conv3dConnection`` with the updates the reference can run on it.  Every attribute is read where the
 reference keeps it (file:line in the comments); state tensors are handed over by pointer and updated in place.
 """
 from __future__ import annotations
@@ -150,6 +151,30 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
         if w.dtype != torch.float32 or not w.is_contiguous():
             raise TypeError("weights must be contiguous float32")
         d.w = w.data_ptr()
+        return
+    if type(conn).__name__ == "Conv3dConnection":
+        # topology.py:847-1025: w [out, in, kd, kh, kw], b [out]; the geometry of F.conv3d (dilation 1: the constructor refuses
+        # any other).  Its rules: learning.NoOp's decay, or PostPre / WeightDependentPostPre with both rates zero (decay and
+        # clamp); the others never run in a learning window (build_net raises the reference's error)
+        d.kind = _abi.SNN_CONN_CONV3D
+        d.cin, d.din, d.hin, d.win = (int(v) for v in conn.source.shape)
+        d.cout, d.dout, d.hout, d.wout = (int(v) for v in conn.target.shape)
+        (d.kd, d.kh, d.kw), (d.sd, d.sh, d.sw), (d.pd, d.ph, d.pw) = conn.kernel_size, conn.stride, conn.padding
+        d.dh = d.dw = 1
+        d.has_norm = int(conn.norm is not None)                                           # topology.py:1004-1018
+        d.norm, d.norm_abs = (_f(conn.norm) if conn.norm is not None else 0.0), 0
+        rule = conn.update_rule
+        name = type(rule).__name__
+        if name in ("NoOp", "PostPre", "WeightDependentPostPre"):
+            d.rule = {"NoOp": _abi.SNN_RULE_NOOP, "PostPre": _abi.SNN_RULE_POSTPRE, "WeightDependentPostPre": _abi.SNN_RULE_WDEP_POSTPRE}[name]
+            d.nu0, d.nu1 = _f(rule.nu[0]), _f(rule.nu[1])
+            d.weight_decay = _f(rule.weight_decay)                                        # learning.py:85
+            d.wmin, d.wmax = _f(conn.wmin), _f(conn.wmax)
+            d.has_clamp = int((math.isfinite(d.wmin) or math.isfinite(d.wmax)) and name != "NoOp")   # learning.py:97-104
+        for t in (conn.w, conn.b):
+            if t.dtype != torch.float32 or not t.is_contiguous():
+                raise TypeError("weights and bias must be contiguous float32")
+        d.w, d.b = conn.w.data_ptr(), conn.b.data_ptr()
         return
     if hasattr(conn, "pipeline"):
         # MulticompartmentConnection (topology.py:402-537) with one Weight feature (topology_features.py:575-671) and at most
@@ -296,6 +321,15 @@ def build_net(network, inputs: Dict[str, torch.Tensor], T: int, B: int):
             # the reference fails in the first step's update: learning.NoOp.update scales connection.w (learning.py:87-94)
             raise AttributeError("'MaxPool2dConnection' object has no attribute 'w' (run MaxPool2dConnection networks with "
                                  "learning off)")
+        if network.learning and type(conn).__name__ == "Conv3dConnection":
+            rule = conn.update_rule
+            name = type(rule).__name__
+            stdp = name in ("PostPre", "WeightDependentPostPre")
+            if (name != "NoOp" and not stdp) or (stdp and bool(rule.nu[0] != 0)):
+                # learning.py:499-559, 978-1050, 1382-1438, 2017-2121, 2739-2855: the bool unfolded source meets torch.bmm
+                raise RuntimeError("expected m1 and m2 to have the same dtype, but got: float != bool")
+            if stdp and bool(rule.nu[1] != 0):
+                raise NotImplementedError(f"{name} with only a post-synaptic rate on a Conv3dConnection")
         # the source is connection.source (network.py:226-248): ann_to_snn's keys need not name it
         src = next((k for k, layer in enumerate(layers) if layer is conn.source), None)
         fill_connection(net.conns[i], conn, names.index(s) if src is None else src, names.index(t), float(network.dt), keep, B=B,

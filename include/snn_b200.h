@@ -100,6 +100,19 @@ extern "C" {
                               reference reshapes that view to [P, cin * K]; for cin = 1 it is the receptive field).
                               normalize: each row of w viewed as [cin * n, K] scaled by norm / (its sum, ascending k),
                               no guard against a zero sum.  Generic tier only, not with SNN_CONN_SPARSE or MCC features */
+#define SNN_CONN_CONV3D 6  /* Conv3dConnection: F.conv3d(s.float(), w, b, stride, padding), topology.py:847-1025.
+                              Source [cin,din,hin,win], target [cout,dout,hout,wout], both row-major; w is
+                              [cout,cin,kd,kh,kw], b is [cout].  The conv fields keep the H and W axes (dh = dw = 1: the
+                              reference refuses dilation); din, dout, kd, sd, pd (which share storage with the
+                              SNN_CONN_SPARSE fields) the depth axis.  Each output size is (in - k + 2p) / s + 1 >= 1.
+                              Target (co, oz, oy, ox) receives the sum of the taps whose zero-padded input position
+                              spiked, in ascending (ci, kz, ky, kx) order from +0, then + b[co].  Rules: SNN_RULE_NONE,
+                              SNN_RULE_NOOP (decay), and SNN_RULE_POSTPRE / WDEP_POSTPRE with nu0 = nu1 = 0 (decay, then
+                              the clamp) — the reference's conv3d rules fail on any pre-synaptic term and pair the
+                              post-synaptic one through transposed kernel axes, so a learning window with any other
+                              rule is SNN_ERR_UNSUPPORTED.  normalize: each row of w viewed as [cout * cin, kd*kh*kw]
+                              scaled by norm / (its sum, ascending), no guard against a zero sum.  No mask.  Generic
+                              tier only, not with SNN_CONN_SPARSE or MCC features */
 
 /* ---- learning rules ---- */
 #define SNN_RULE_NONE 0        /* MCC_learning.NoOp: update() does nothing    MCC_learning.py:120-146 */
@@ -244,10 +257,19 @@ typedef struct snn_conn {
     float e_trace_decay, tc_e_trace, et_coef;
     /* SNN_CONN_SPARSE: compressed sparse rows of the [n_src, n_tgt] pattern.  sp_rowptr [n_src + 1], monotone, in
        [0, nnz]; sp_col [nnz], strictly ascending within a row, < n_tgt; w [nnz] the values in the same order, decayed
-       in place by SNN_RULE_NOOP.  A malformed pattern is reported as SNN_ERR_BAD_ARG (in *err_flag by the window). */
-    const int32_t *sp_rowptr;
-    const int32_t *sp_col;
-    int32_t nnz;
+       in place by SNN_RULE_NOOP.  A malformed pattern is reported as SNN_ERR_BAD_ARG (in *err_flag by the window).
+       SNN_CONN_CONV3D (topology.py:847-1025) keeps its depth axis in the same storage: source depth din, target depth
+       dout, kernel depth kd, stride sd, padding pd.  A connection is never both, so the layout is the one without it. */
+    union {
+        struct {
+            const int32_t *sp_rowptr;
+            const int32_t *sp_col;
+            int32_t nnz;
+        };
+        struct {
+            int32_t din, dout, kd, sd, pd;
+        };
+    };
     /* SNN_CONN_MCC with Probability / Mask / Intensity features besides its Weight (topology.py:437-479).  Each is an
        [n_src, n_tgt] row-major matrix or NULL (feature absent).  A spiking source i adds fl(w[i,j] * f_int[i,j]) (just
        w[i,j] without f_int) to target j when f_mask[i,j] != 0 and the Probability draw of synapse (i, j) transmits

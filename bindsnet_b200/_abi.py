@@ -21,6 +21,7 @@ SNN_RULE_MSTDPET = 7
 SNN_REDUCE_SUM, SNN_REDUCE_MEAN = 0, 1
 SNN_EXT_NONE, SNN_EXT_U8, SNN_EXT_F32 = 0, 1, 2
 SNN_W_DENSE, SNN_W_DIAG, SNN_W_OFFDIAG = 0, 1, 2
+SNN_SYN_FULL, SNN_SYN_TGT, SNN_SYN_SRC, SNN_SYN_ONE = 1, 2, 3, 4
 
 SNN_OK = 0
 SNN_ERR_BAD_ARG = 1
@@ -104,8 +105,25 @@ class _SparseOrConv3d(C.Union):
     _fields_ = [("_sparse", _SparseFields), ("_conv3d", _Conv3dFields)]
 
 
+class _FeatureFields(C.Structure):
+    _fields_ = [("f_prob", C.c_void_p), ("f_mask", C.c_void_p), ("f_int", C.c_void_p),
+                ("draw_seed", C.c_uint32), ("draw_step", C.c_uint32), ("draw_conn", C.c_uint32)]
+
+
+class _SynapseFields(C.Structure):
+    _fields_ = [("wmin_t", C.c_void_p), ("wmax_t", C.c_void_p), ("nu0_t", C.c_void_p), ("nu1_t", C.c_void_p),
+                ("wmin_form", C.c_int8), ("wmax_form", C.c_int8), ("nu0_form", C.c_int8), ("nu1_form", C.c_int8)]
+
+
+class _FeaturesOrSynapse(C.Union):
+    """The storage SNN_CONN_MCC's features and SNN_CONN_DENSE's per-synapse tensors share (a connection is never both)."""
+
+    _anonymous_ = ("_feat", "_syn")
+    _fields_ = [("_feat", _FeatureFields), ("_syn", _SynapseFields)]
+
+
 class SnnConn(C.Structure):
-    _anonymous_ = ("_u",)
+    _anonymous_ = ("_u", "_f")
     _fields_ = [
         ("kind", C.c_int32),
         ("src", C.c_int32),
@@ -146,12 +164,7 @@ class SnnConn(C.Structure):
         ("tc_e_trace", C.c_float),
         ("et_coef", C.c_float),
         ("_u", _SparseOrConv3d),
-        ("f_prob", C.c_void_p),
-        ("f_mask", C.c_void_p),
-        ("f_int", C.c_void_p),
-        ("draw_seed", C.c_uint32),
-        ("draw_step", C.c_uint32),
-        ("draw_conn", C.c_uint32),
+        ("_f", _FeaturesOrSynapse),
         ("pool_rates", C.c_void_p),
         ("pool_decay", C.c_float),
     ]

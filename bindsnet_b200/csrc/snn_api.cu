@@ -89,7 +89,12 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
         if (SNN_RULE_IS_STDP(C.rule) && (!net->layers[C.src].traces || !net->layers[C.tgt].traces))
             return SNN_ERR_BAD_ARG;
         if (C.mask && (C.kind != SNN_CONN_DENSE || SNN_RULE_IS_MSTDP(C.rule))) return SNN_ERR_UNSUPPORTED;
-        if ((C.f_prob || C.f_mask || C.f_int) && C.kind != SNN_CONN_MCC) return SNN_ERR_BAD_ARG;
+        // the feature storage holds a dense connection's per-synapse tensors (snn_b200.h); any other kind leaves it empty
+        if ((C.f_prob || C.f_mask || C.f_int) && C.kind != SNN_CONN_MCC && C.kind != SNN_CONN_DENSE) return SNN_ERR_BAD_ARG;
+        if (snn_has_syn(C)) {
+            const int rc = snn_syn_check(C);
+            if (rc != SNN_OK) return rc;
+        }
         // a PassThroughNodes layer carries 0 / 1 spikes: pooled ones in, none of a rule's traces (snn_b200.h)
         const bool pass_src = net->layers[C.src].kind == SNN_NODE_PASSTHROUGH, pass_tgt = net->layers[C.tgt].kind == SNN_NODE_PASSTHROUGH;
         if (pass_tgt && !pool) return SNN_ERR_UNSUPPORTED;
@@ -119,8 +124,15 @@ static bool has_sparse(const snn_net_t *net) {
 static bool has_feat(const snn_net_t *net) {
     for (int c = 0; c < net->n_conns; ++c) {
         const snn_conn_t &C = net->conns[c];
-        if (C.f_prob || C.f_mask || C.f_int) return true;
+        if (C.kind == SNN_CONN_MCC && (C.f_prob || C.f_mask || C.f_int)) return true;
     }
+    return false;
+}
+
+// some dense connection carries per-synapse bounds or rates (snn_b200.h)
+static bool has_syn(const snn_net_t *net) {
+    for (int c = 0; c < net->n_conns; ++c)
+        if (snn_has_syn(net->conns[c])) return true;
     return false;
 }
 
@@ -222,9 +234,11 @@ int snn_b200_select_tier(const snn_net_t *net, const snn_run_opts_t *opts) {
     if (validate(net, opts) != SNN_OK) return 0;
     // one extra instantiation of the generic kernel each for sparse, feature and pooling plans (pooling: also plans with
     // a LocalConnection2D, a Conv3dConnection, SubtractiveResetIFNodes or PassThroughNodes), not combinations
-    if ((int)has_sparse(net) + (int)has_feat(net) + (int)has_pool(net) > 1) return 0;
-    // the fused DiehlAndCook2015 kernels (and so the delta windows) have neither the sparse, the feature nor the pooling gather
-    if (has_sparse(net) || has_feat(net) || has_pool(net))
+    // (and one for plans with per-synapse bounds or rates)
+    if ((int)has_sparse(net) + (int)has_feat(net) + (int)has_pool(net) + (int)has_syn(net) > 1) return 0;
+    // the fused DiehlAndCook2015 kernels (and so the delta windows) have neither the sparse, the feature nor the pooling
+    // gather, and read scalar bounds and rates only
+    if (has_sparse(net) || has_feat(net) || has_pool(net) || has_syn(net))
         return (opts->tier == 0 || opts->tier == 1) && !opts->delta_w && !opts->delta_theta ? 1 : 0;
     if (opts->delta_w || opts->delta_theta)   // delta windows exist in the barrier kernel only
         return (opts->tier == 0 || opts->tier == 2) && snn_fused_dc_supported(net, opts) ? 2 : 0;
@@ -241,7 +255,7 @@ int snn_b200_select_tier(const snn_net_t *net, const snn_run_opts_t *opts) {
 size_t snn_b200_workspace_bytes(const snn_net_t *net, const snn_run_opts_t *opts) {
     if (validate(net, opts) != SNN_OK) return 0;
     size_t g = layout_generic(net, opts, nullptr, nullptr);
-    if (has_sparse(net) || has_feat(net) || has_pool(net)) return g;
+    if (has_sparse(net) || has_feat(net) || has_pool(net) || has_syn(net)) return g;
     size_t f = snn_fused_dc_supported(net, opts) ? snn_fused_dc_workspace_bytes(net, opts) : 0;
     size_t f2 = snn_fused_dc2_supported(net, opts) ? snn_fused_dc2_workspace_bytes(net, opts) : 0;
     if (f2 > f) f = f2;
@@ -278,7 +292,7 @@ int snn_b200_run_window(const snn_net_t *net, const snn_run_opts_t *opts, void *
         N.conns[c] = net->conns[c];
         const snn_conn_t &C = net->conns[c];
         if (C.mask) N.any_mask = 1;
-        if (C.f_prob || C.f_mask || C.f_int) N.any_feat = 1;
+        if (C.kind == SNN_CONN_MCC && (C.f_prob || C.f_mask || C.f_int)) N.any_feat = 1;
     }
     N.any_pool = has_pool(net) ? 1 : 0;
     if (cudaMemsetAsync(N.bar, 0, sizeof(unsigned int) * 96, stream) != cudaSuccess) return SNN_ERR_CUDA;

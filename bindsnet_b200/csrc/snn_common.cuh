@@ -160,6 +160,19 @@ static inline bool snn_conv3d_rule_ok(const snn_conn_t &C) {
     return (C.rule == SNN_RULE_POSTPRE || C.rule == SNN_RULE_WDEP_POSTPRE) && C.nu0 == 0.0f && C.nu1 == 0.0f;
 }
 
+// The per-synapse tensors of a dense connection (snn_b200.h): known forms, the rate pair set together, PostPre's rates
+// broadcast to [1, n_tgt] (any other shape is the reference's bmm error), and no MCC-only rule.
+static inline int snn_syn_check(const snn_conn_t &C) {
+    auto form_ok = [](const float *t, int f) { return !t || (f >= SNN_SYN_FULL && f <= SNN_SYN_ONE); };
+    if (!form_ok(C.wmin_t, C.wmin_form) || !form_ok(C.wmax_t, C.wmax_form) || !form_ok(C.nu0_t, C.nu0_form) || !form_ok(C.nu1_t, C.nu1_form))
+        return SNN_ERR_BAD_ARG;
+    if ((C.nu0_t == nullptr) != (C.nu1_t == nullptr) || C.rule == SNN_RULE_MCC_POSTPRE) return SNN_ERR_BAD_ARG;
+    if (C.rule == SNN_RULE_POSTPRE && C.nu0_t && ((C.nu0_form != SNN_SYN_TGT && C.nu0_form != SNN_SYN_ONE) ||
+                                                  (C.nu1_form != SNN_SYN_TGT && C.nu1_form != SNN_SYN_ONE)))
+        return SNN_ERR_BAD_ARG;
+    return SNN_OK;
+}
+
 __host__ __device__ __forceinline__ int pool_rate_slot(int T, int t) { return (T - 1 - t) & 1; }
 __device__ __forceinline__ float *pool_rates_at(const DevNet &N, int c, int slot) { return slot ? N.pool_r1[c] : N.conns[c].pool_rates; }
 // MaxPool2dConnection.compute step 1 (topology.py:1175-1176): r -= decay * r; r += s
@@ -354,6 +367,39 @@ __device__ __forceinline__ float apply_rule(const snn_conn_t &C, float w, float 
     }
     if (C.weight_decay != 0.0f) w = w * C.weight_decay;
     if (C.has_clamp) w = clampf(w, C.wmin, C.wmax);
+    return w;
+}
+
+// A dense connection's per-synapse tensors (snn_b200.h wmin_t / wmax_t / nu0_t / nu1_t).  Plans that hold one run the
+// SYN instantiation of the learning phase; the others never read these fields.
+__host__ __device__ inline bool snn_has_syn(const snn_conn_t &C) {
+    return C.kind == SNN_CONN_DENSE && (C.wmin_t || C.wmax_t || C.nu0_t || C.nu1_t);
+}
+// element (i, j) of a tensor in broadcast form `form`, or the scalar when there is no tensor
+__device__ __forceinline__ float syn_at(const float *t, int form, float scalar, int i, int j, int nt) {
+    if (!t) return scalar;
+    const size_t k = form == SNN_SYN_FULL ? (size_t)i * nt + j : form == SNN_SYN_TGT ? (size_t)j : form == SNN_SYN_SRC ? (size_t)i : 0;
+    return __ldg(t + k);
+}
+// apply_rule with the bounds and rates of synapse (i, j).  POSTPRE's rates are inside U / V already (the staged
+// fl(x_tgt * nu0[j]) and x_src * nu1[j]); HEBBIAN's gates are 1 (snn_b200.h), so its rates apply ungated like the
+// reference's.
+__device__ __forceinline__ float apply_rule_syn(const snn_conn_t &C, float w, float U, bool pre_t, float V, bool post_t, int i, int j,
+                                                int nt) {
+    if (C.rule == SNN_RULE_WDEP_POSTPRE) {
+        float upd = 0.0f;
+        if (C.nu0 != 0.0f) upd = upd - (syn_at(C.nu0_t, C.nu0_form, C.nu0, i, j, nt) * (pre_t ? U : 0.0f)) * (w - syn_at(C.wmin_t, C.wmin_form, C.wmin, i, j, nt));
+        if (C.nu1 != 0.0f) upd = upd + (syn_at(C.nu1_t, C.nu1_form, C.nu1, i, j, nt) * (post_t ? V : 0.0f)) * (syn_at(C.wmax_t, C.wmax_form, C.wmax, i, j, nt) - w);
+        w = w + upd;
+    } else if (C.rule == SNN_RULE_POSTPRE) {
+        if (pre_t) w = w - U;
+        if (post_t) w = w + V;
+    } else if (C.rule == SNN_RULE_HEBBIAN) {
+        if (C.nu0 != 0.0f) w = w + syn_at(C.nu0_t, C.nu0_form, C.nu0, i, j, nt) * (pre_t ? U : 0.0f);
+        if (C.nu1 != 0.0f) w = w + syn_at(C.nu1_t, C.nu1_form, C.nu1, i, j, nt) * (post_t ? V : 0.0f);
+    }
+    if (C.weight_decay != 0.0f) w = w * C.weight_decay;
+    if (C.has_clamp) w = clampf(w, syn_at(C.wmin_t, C.wmin_form, C.wmin, i, j, nt), syn_at(C.wmax_t, C.wmax_form, C.wmax, i, j, nt));
     return w;
 }
 

@@ -61,7 +61,9 @@ __device__ __forceinline__ void sparse_unit(const DevNet &N, int u, int &c, int 
 // combined with SPARSE or FEAT.  The
 // barriers are those of the plain window: the rates a gather reads were written before the barrier that ends the previous
 // step (or, in one-step mode, before the barrier that ends the source layer).
-template <int CTAS, bool SPARSE, bool FEAT, bool POOL>
+// SYN: some dense connection carries per-synapse bounds or rates (snn_b200.h); only the learning phase differs, and
+// plans without them run the instantiation whose code never reads those fields.  Not combined with SPARSE, FEAT or POOL.
+template <int CTAS, bool SPARSE, bool FEAT, bool POOL, bool SYN = false>
 __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(const __grid_constant__ DevNet N) {
 #ifdef SNN_EMU
     float *smem = emu::tls_cta->dyn_smem;
@@ -187,11 +189,11 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                 const snn_conn_t &C = N.conns[c];
                 const int v = u - N.p3_first[c];
                 if (SNN_RULE_IS_MSTDP(C.rule)) {   // dense MSTDP / MSTDPET: by source tiles
-                    phase3_mstdp_dense(N, c, v, t, M);
+                    phase3_mstdp_dense<SYN>(N, c, v, t, M);
                 } else {
                     const int rcn = N.p3_rc[c], tile = v / rcn, rc = v - tile * rcn;
                     const int nwS = N.layers[C.src].nw;
-                    phase3(N, c, tile, (int)((long long)rc * nwS / rcn), (int)((long long)(rc + 1) * nwS / rcn), t, M);
+                    phase3<SYN>(N, c, tile, (int)((long long)rc * nwS / rcn), (int)((long long)(rc + 1) * nwS / rcn), t, M);
                 }
             }
             GPROF(4)
@@ -308,6 +310,8 @@ int snn_generic_launch(DevNet &N, cudaStream_t) {
     if (N.sp_units) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, true, false, false>(*(const DevNet *)a); }, &N);
     else if (N.any_feat) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, true, false>(*(const DevNet *)a); }, &N);
     else if (N.any_pool) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, true>(*(const DevNet *)a); }, &N);
+    else if (std::any_of(N.conns, N.conns + N.n_conns, snn_has_syn))
+        emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, false, true>(*(const DevNet *)a); }, &N);
     else emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, false>(*(const DevNet *)a); }, &N);
     return 0;
 }
@@ -323,10 +327,12 @@ int snn_generic_launch(DevNet &N, cudaStream_t stream) {
     // two CTAs per SM unless SNN_B200_GVAR=3 asks for the spilling three-CTA experiment (plans without a SparseConnection,
     // MCC features or the POOL instantiation's kinds)
     const bool sparse = std::any_of(N.conns, N.conns + N.n_conns, [](const snn_conn_t &C) { return C.kind == SNN_CONN_SPARSE; });
+    const bool syn = std::any_of(N.conns, N.conns + N.n_conns, snn_has_syn);
     bool three = false;
-    if (const char *v = getenv("SNN_B200_GVAR")) three = !sparse && !N.any_feat && !N.any_pool && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
+    if (const char *v = getenv("SNN_B200_GVAR")) three = !sparse && !N.any_feat && !N.any_pool && !syn && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
     const void *kern = three ? (const void *)snn_generic_window<3, false, false, false>
                      : sparse ? (const void *)snn_generic_window<2, true, false, false>
+                     : syn ? (const void *)snn_generic_window<2, false, false, false, true>
                      : N.any_feat ? (const void *)snn_generic_window<2, false, true, false>
                      : N.any_pool ? (const void *)snn_generic_window<2, false, false, true> : (const void *)snn_generic_window<2, false, false, false>;
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

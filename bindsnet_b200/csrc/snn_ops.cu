@@ -208,10 +208,11 @@ __global__ void pack_bits_kernel(const uint8_t *__restrict__ s, uint32_t *__rest
     if (lane == 0) bits[(size_t)b * nw + w] = word;
 }
 
+template <bool SYN>
 __global__ void __launch_bounds__(SNN_GEN_THREADS) conn_update_kernel(const __grid_constant__ DevNet N, int ci) {
     SNN_DYN_SHARED(float, smem);
     const GenSmem M = gen_carve(smem, N.B);
-    phase3(N, ci, blockIdx.x, 0, N.layers[N.conns[ci].src].nw, 0, M);
+    phase3<SYN>(N, ci, blockIdx.x, 0, N.layers[N.conns[ci].src].nw, 0, M);
 }
 
 __global__ void __launch_bounds__(SNN_GEN_THREADS) conn_normalize_kernel(snn_conn_t C, int ns, int nt) {
@@ -276,8 +277,9 @@ int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, 
     if (!conn || (!conn->w && !(conn->kind == SNN_CONN_SPARSE && conn->nnz == 0) && conn->kind != SNN_CONN_MAXPOOL2D) || !s || !out ||
         n_src <= 0 || n_tgt <= 0 || B <= 0)
         return SNN_ERR_BAD_ARG;
-    const bool feat = conn->f_prob || conn->f_mask || conn->f_int;
-    if (feat && conn->kind != SNN_CONN_MCC) return SNN_ERR_BAD_ARG;
+    // (on SNN_CONN_DENSE this storage holds the per-synapse tensors, which the gather does not read)
+    const bool feat = conn->kind == SNN_CONN_MCC && (conn->f_prob || conn->f_mask || conn->f_int);
+    if (conn->kind != SNN_CONN_MCC && conn->kind != SNN_CONN_DENSE && (conn->f_prob || conn->f_mask || conn->f_int)) return SNN_ERR_BAD_ARG;
     if (conn->kind == SNN_CONN_MAXPOOL2D) {   // updates conn->pool_rates [B, n_src] in place, then writes [B, n_tgt]
         const int rc = snn_pool_geometry_ok(*conn, n_src, n_tgt);
         if (rc != SNN_OK || conn->b) return rc != SNN_OK ? rc : SNN_ERR_BAD_ARG;
@@ -360,6 +362,11 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
         if (C.rule == SNN_RULE_MCC_POSTPRE) return SNN_ERR_UNSUPPORTED;
     }
     if (SNN_RULE_IS_MSTDP(C.rule)) return SNN_ERR_UNSUPPORTED;
+    const bool syn = snn_has_syn(C);
+    if (syn) {
+        const int rc = snn_syn_check(C);
+        if (rc != SNN_OK) return rc;
+    }
     if (C.rule == SNN_RULE_NONE) return SNN_OK;
     cudaStream_t stream = (cudaStream_t)stream_;
     DevNet N;
@@ -389,8 +396,13 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
         return cuda_rc(cudaGetLastError());
     }
     const size_t smem = gen_smem_bytes(B);
-    cudaFuncSetAttribute(conn_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    SNN_LAUNCH(conn_update_kernel, N.layers[C.tgt].nw, SNN_GEN_THREADS, smem, stream, N, ci);
+    if (syn) {
+        cudaFuncSetAttribute(conn_update_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        SNN_LAUNCH(conn_update_kernel<true>, N.layers[C.tgt].nw, SNN_GEN_THREADS, smem, stream, N, ci);
+    } else {
+        cudaFuncSetAttribute(conn_update_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        SNN_LAUNCH(conn_update_kernel<false>, N.layers[C.tgt].nw, SNN_GEN_THREADS, smem, stream, N, ci);
+    }
     return cuda_rc(cudaGetLastError());
 }
 

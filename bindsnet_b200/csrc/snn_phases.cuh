@@ -853,6 +853,9 @@ __device__ void phase2(const DevNet &N, int li, int tile, int chunk, int t) {
 // (every row group reads them), a warp owns one group of 32 source rows at a time, stages the pre-synaptic
 // traces of the (few) samples with a post-synaptic event for those rows, and rewrites the rows eight at a time
 // so that eight weight loads are in flight.
+// SYN: the connection may carry per-synapse bounds and rates (snn_b200.h wmin_t ...); plans without them run the
+// instantiation that never reads those fields.
+template <bool SYN>
 __device__ void phase3(const DevNet &N, int ci, int tile, int wg0, int wg1, int t, const GenSmem &M) {
     const snn_conn_t &C = N.conns[ci];
     const DevLayer &S = N.layers[C.src], &G = N.layers[C.tgt];
@@ -869,6 +872,8 @@ __device__ void phase3(const DevNet &N, int ci, int tile, int wg0, int wg1, int 
     const bool full = decay_on || (C.has_clamp && t == 0);
     const float Bf = (float)B;
     const bool stage = pre_on && M.xt != nullptr;
+    // PostPre's pre-synaptic rate of my column (per target only, snn_b200.h)
+    const float nu0j = SYN ? syn_at(C.nu0_t, C.nu0_form, C.nu0, 0, valid ? j : 0, nt) : C.nu0;
 
     // Samples whose target-trace row is all zero in this tile cannot change the pre-synaptic term (adding +-0 to a sum
     // that started at +0 is a bitwise no-op), and in networks of rarely spiking neurons that is most of them: the
@@ -887,7 +892,7 @@ __device__ void phase3(const DevNet &N, int ci, int tile, int wg0, int wg1, int 
             for (int q = 0; q < 8; ++q) {
                 const int b = b0 + q * SNN_GEN_WARPS;
                 if (b < B) {
-                    const float v = wdep ? tx[q] : tx[q] * C.nu0;
+                    const float v = wdep ? tx[q] : tx[q] * nu0j;
                     M.xt[b * 32 + lane] = v;
                     const bool nzrow = __any_sync(0xffffffffu, v != 0.0f);
                     if (lane == 0 && nzrow) atomicOr(M.live + (b >> 5), 1u << (b & 31));
@@ -997,7 +1002,7 @@ __device__ void phase3(const DevNet &N, int ci, int tile, int wg0, int wg1, int 
                         } else {
                             if (valid) {
                                 tx = __ldcg(G.L.x + (size_t)b * nt + j);
-                                if (!wdep) tx = tx * C.nu0;
+                                if (!wdep) tx = tx * nu0j;
                             }
                             if (!__any_sync(0xffffffffu, tx != 0.0f)) continue;
                         }
@@ -1026,6 +1031,7 @@ __device__ void phase3(const DevNet &N, int ci, int tile, int wg0, int wg1, int 
                     U = acc[lane * 32 + jl];
                     if (C.reduction == SNN_REDUCE_MEAN) U = U / Bf;
                 }
+                const float nu1c = SYN ? syn_at(C.nu1_t, C.nu1_form, C.nu1, 0, jc, nt) : C.nu1;
                 for (int g = 0; g < NG; ++g) {
                     uint32_t m = M.colmask[g * 32 + jl];
                     while (m) {
@@ -1033,12 +1039,12 @@ __device__ void phase3(const DevNet &N, int ci, int tile, int wg0, int wg1, int 
                         m &= m - 1;
                         const int slot = M.evslot[b];
                         const float xs = slot != 0xFF ? xsw[slot * 32 + lane] : __ldcg(S.xpub + ((size_t)wr * B + b) * ns + i);
-                        V = V + xs * (wdep ? 1.0f : C.nu1);
+                        V = V + xs * (wdep ? 1.0f : nu1c);
                     }
                 }
                 if (C.reduction == SNN_REDUCE_MEAN) V = V / Bf;
                 float *wp = C.w + (size_t)i * nt + jc;
-                *wp = apply_rule(C, __ldcg(wp), U, pre_t, V, true);
+                *wp = SYN ? apply_rule_syn(C, __ldcg(wp), U, pre_t, V, true, i, jc, nt) : apply_rule(C, __ldcg(wp), U, pre_t, V, true);
             }
         }
         __syncwarp();
@@ -1073,7 +1079,8 @@ __device__ void phase3(const DevNet &N, int ci, int tile, int wg0, int wg1, int 
                             U = acc[r * 32 + lane];
                             if (C.reduction == SNN_REDUCE_MEAN) U = U / Bf;
                         }
-                        C.w[(size_t)i * nt + j] = apply_rule(C, wv[q], U, pre_t, 0.0f, false);
+                        C.w[(size_t)i * nt + j] = SYN ? apply_rule_syn(C, wv[q], U, pre_t, 0.0f, false, i, j, nt)
+                                                      : apply_rule(C, wv[q], U, pre_t, 0.0f, false);
                     }
                 }
             }
@@ -1107,7 +1114,8 @@ __device__ __forceinline__ bool bit_of(const uint32_t *row, int i) { return (__l
 // lane) x all columns j (warps stride over them); the batch sum runs in ascending b per (i, j).  When it
 // fits, the rule state the batch loop reads (p_plus and the pre-synaptic spikes of the unit's rows, p_minus
 // and the post-synaptic spikes of all columns) is staged in shared memory first, so that the B-long
-// dependent loop never waits for L2.
+// dependent loop never waits for L2.  SYN: as for phase3.
+template <bool SYN>
 __device__ void phase3_mstdp_dense(const DevNet &N, int ci_, int tile, int t, const GenSmem &GS) {
     const snn_conn_t &C = N.conns[ci_];
     const DevMstdp &M = N.mst[ci_];
@@ -1171,9 +1179,12 @@ __device__ void phase3_mstdp_dense(const DevNet &N, int ci_, int tile, int t, co
                 float et = __ldcg(C.e_trace + (size_t)i * nt + j) * C.e_trace_decay;   // :2229
                 et = et + e / C.tc_e_trace;                                            // :2230
                 C.e_trace[(size_t)i * nt + j] = et;
-                float x = __ldcg(C.w + (size_t)i * nt + j) + C.et_coef * et;           // :2232-2238
+                // :2232-2238; a rate tensor is scaled per element, ((nu0 * dt) * reward) * e_trace left to right
+                const float coef = SYN && C.nu0_t ? (syn_at(C.nu0_t, C.nu0_form, 0.0f, i, j, nt) * C.dt_scale) * C.reward : C.et_coef;
+                float x = __ldcg(C.w + (size_t)i * nt + j) + coef * et;
                 if (C.weight_decay != 0.0f) x = x * C.weight_decay;
-                if (C.has_clamp) x = clampf(x, C.wmin, C.wmax);
+                if (C.has_clamp) x = SYN ? clampf(x, syn_at(C.wmin_t, C.wmin_form, C.wmin, i, j, nt), syn_at(C.wmax_t, C.wmax_form, C.wmax, i, j, nt))
+                                         : clampf(x, C.wmin, C.wmax);
                 C.w[(size_t)i * nt + j] = x;
             }
     } else if (i < ns)
@@ -1195,9 +1206,10 @@ __device__ void phase3_mstdp_dense(const DevNet &N, int ci_, int tile, int t, co
                 }
             }
             if (C.reduction == SNN_REDUCE_MEAN) upd = upd / Bf;
-            float x = __ldcg(C.w + (size_t)i * nt + j) + C.nu0 * upd;
+            float x = __ldcg(C.w + (size_t)i * nt + j) + (SYN ? syn_at(C.nu0_t, C.nu0_form, C.nu0, i, j, nt) : C.nu0) * upd;
             if (C.weight_decay != 0.0f) x = x * C.weight_decay;
-            if (C.has_clamp) x = clampf(x, C.wmin, C.wmax);
+            if (C.has_clamp) x = SYN ? clampf(x, syn_at(C.wmin_t, C.wmin_form, C.wmin, i, j, nt), syn_at(C.wmax_t, C.wmax_form, C.wmax, i, j, nt))
+                                     : clampf(x, C.wmin, C.wmax);
             C.w[(size_t)i * nt + j] = x;
         }
     // P+ and the pre-synaptic spikes of this step for my rows; tile 0 also does P- and the post side

@@ -59,7 +59,10 @@ class ShardedWindowRunner:
                 d.norm = float(conn.norm) if conn.norm is not None else 0.0
                 d.norm_abs = 1
                 import math
-                d.wmin, d.wmax = float(conn.wmin), float(conn.wmax)
+                if (conn.wmin.numel() != 1 or conn.wmax.numel() != 1) and code >= _abi.SNN_RULE_POSTPRE:
+                    raise NotImplementedError("the multi-GPU combine clamps with scalar bounds: a learned connection with "
+                                              "per-synapse wmin / wmax tensors is not supported by ShardedWindowRunner")
+                d.wmin, d.wmax = (float(conn.wmin), float(conn.wmax)) if conn.wmin.numel() == 1 and conn.wmax.numel() == 1 else (-math.inf, math.inf)
                 d.has_clamp = int(code >= _abi.SNN_RULE_POSTPRE and (math.isfinite(d.wmin) or math.isfinite(d.wmax)))
             if d.rule >= _abi.SNN_RULE_POSTPRE or d.has_norm:
                 # [Cout,Cin,kh,kw] / [Cout,Cin,kd,kh,kw] weights normalise per filter (topology.py:824-837, 1004-1018), the

@@ -214,7 +214,10 @@ class _EligibilityTrace(_RewardModulated):
         d.e_trace_decay = float(torch.exp(-dt / self.tc_e_trace))          # learning.py:2229
         d.tc_e_trace = float(self.tc_e_trace)
         # update = nu[0] * dt * reward * eligibility_trace (learning.py:2232): the scalar product in fp32, left to right
-        d.et_coef = float(self.nu[0].float() * dt * float(self._run_kwargs["reward"]))
+        if getattr(self, "_nu_tensors", False):   # per-synapse rates: the kernel scales each one (snn_b200.h)
+            d.et_coef = 0.0
+        else:
+            d.et_coef = float(self.nu[0].float() * dt * float(self._run_kwargs["reward"]))
 
 
 class MSTDP(_RewardModulated, MCC_LearningRule):

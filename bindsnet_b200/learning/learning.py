@@ -44,7 +44,15 @@ class LearningRule(ABC):
         elif all(isinstance(e, (float, int)) for e in nu):
             self.nu = torch.tensor(nu, dtype=torch.float)
         else:
-            raise NotImplementedError("per-synapse learning-rate tensors are not supported by the CUDA core yet")
+            # a pair of tensors (learning.py:66): per-neuron or per-synapse rates, on a dense Connection only
+            from ..network.topology import Connection
+
+            if not isinstance(connection, Connection) or not connection._synapse_tensors:
+                raise NotImplementedError(f"per-synapse learning-rate tensors are not supported by the CUDA core on a "
+                                          f"{type(connection).__name__} (dense Connection only)")
+            self.nu = torch.stack(tuple(nu), dim=0).to(dtype=torch.float)
+        # rates the kernels read from the tensor (0-d rates are scalars, read once per version of the tensor)
+        self._nu_tensors = self.nu.dim() > 1
         if not self.nu.any() and not isinstance(self, NoOp):
             warnings.warn(
                 f"nu is set to zeros for {type(self).__name__} learning rule. "
@@ -70,7 +78,7 @@ class LearningRule(ABC):
                 w *= self.weight_decay
             wmin, wmax = self.connection.wmin, self.connection.wmax       # learning.py:97-104
             if bool((wmin != -np.inf).any()) or bool((wmax != np.inf).any()):
-                w.clamp_(float(wmin), float(wmax))
+                w.clamp_(wmin, wmax)
             return
         from ..network import _plan
 
@@ -84,14 +92,17 @@ class LearningRule(ABC):
             )
         d.rule = self.rule_code
         d.reduction = self._reduction_code
-        d.nu0 = float(self.nu[0])
-        d.nu1 = float(self.nu[1])
+        if self._nu_tensors:   # Connection._fill_desc points the kernels at the tensors and sets the gates
+            d.nu0 = d.nu1 = 0.0
+        else:
+            d.nu0 = float(self.nu[0])
+            d.nu1 = float(self.nu[1])
         d.weight_decay = float(self.weight_decay)
-        # learning.py:97-104: clamp iff a bound is finite and the rule is not NoOp
-        from ..network.nodes import _scalar
+        # learning.py:97-104: clamp iff some element of wmin is not -inf or some element of wmax is not +inf, and the
+        # rule is not NoOp
+        from ..network.topology import bounds_clamp
 
-        finite = _scalar(self.connection.wmin, "wmin") != -np.inf or _scalar(self.connection.wmax, "wmax") != np.inf
-        d.has_clamp = int(finite and not isinstance(self, NoOp))
+        d.has_clamp = int(bounds_clamp(self.connection.wmin, self.connection.wmax) and not isinstance(self, NoOp))
 
 
 def _check_connection(rule, connection) -> None:

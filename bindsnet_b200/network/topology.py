@@ -21,6 +21,111 @@ from .. import _abi
 from .nodes import Nodes, _scalar
 
 
+_TENSOR_FLAGS: dict = {}
+
+
+def _tensor_flag(t: torch.Tensor, tag: str, fn) -> bool:
+    """``fn(t)`` as a host bool, evaluated once per tensor object and version: reading a device tensor synchronises the
+    stream, and building the plan of a window must not stall the window still running on it."""
+    key = (tag, id(t))
+    hit = _TENSOR_FLAGS.get(key)
+    if hit is not None and hit[0] is t and hit[1] == t._version:
+        return hit[2]
+    with torch.no_grad():
+        out = bool(fn(t))
+    if len(_TENSOR_FLAGS) > 4096:
+        _TENSOR_FLAGS.clear()
+    _TENSOR_FLAGS[key] = (t, t._version, out)
+    return out
+
+
+def bounds_clamp(wmin: torch.Tensor, wmax: torch.Tensor) -> bool:
+    """learning.py:97-104: the base update clamps when some element of ``wmin`` is not -inf or some element of ``wmax``
+    is not +inf (scalars or tensors)."""
+    return _tensor_flag(wmin, "lo", lambda t: (t != -np.inf).any()) or _tensor_flag(wmax, "hi", lambda t: (t != np.inf).any())
+
+
+def nu_any(nu: torch.Tensor, k: int) -> bool:
+    """``nu[k].any()`` (the gate of PostPre's and WeightDependentPostPre's terms, learning.py:403, 410, 640, 645)."""
+    return _tensor_flag(nu, f"any{k}", lambda t: t[k].any())
+
+
+def synapse_tensor(t: torch.Tensor, ns: int, nt: int, device: torch.device, name: str, owner=None):
+    """``(tensor, form)``: what the kernels read for a bound or rate tensor that broadcasts to ``w``'s ``[ns, nt]``
+    (include/snn_b200.h SNN_SYN_*).  A per-target ``[nt]`` / ``[1, nt]``, a per-source ``[ns, 1]``, a one-element or a
+    contiguous ``[ns, nt]`` tensor is read in place; any other layout is copied once to a contiguous ``[ns, nt]`` and the
+    copy kept on ``owner`` until the tensor changes."""
+    if t.device != device:
+        raise RuntimeError(f"Expected all tensors to be on the same device, but found at least two devices, {device} and "
+                           f"{t.device}! ({name} is on {t.device}, the weights on {device})")
+    try:
+        ok = tuple(torch.broadcast_shapes(tuple(t.shape), (ns, nt))) == (ns, nt)
+    except RuntimeError:
+        ok = False
+    if not ok:
+        raise RuntimeError(f"The size of {name} {list(t.shape)} does not broadcast to the weights' size [{ns}, {nt}]")
+    if t.dtype != torch.float32:
+        raise TypeError(f"{name} must be float32, got {t.dtype}")
+    e = t.detach().expand(ns, nt)
+    s0 = 0 if ns == 1 else e.stride(0)
+    s1 = 0 if nt == 1 else e.stride(1)
+    form = {(0, 0): _abi.SNN_SYN_ONE, (0, 1): _abi.SNN_SYN_TGT, (1, 0): _abi.SNN_SYN_SRC, (nt, 1): _abi.SNN_SYN_FULL}.get((s0, s1))
+    if form is not None:
+        return e, form
+    key = (t.data_ptr(), t._version, tuple(t.shape), tuple(t.stride()))
+    cache = owner.__dict__.setdefault("_b200_syn_copies", {}) if owner is not None else {}
+    hit = cache.get(name)
+    if hit is None or hit[0] != key:
+        hit = (key, e.contiguous(), t)
+        cache[name] = hit
+    return hit[1], _abi.SNN_SYN_FULL
+
+
+def fill_synapse_tensors(d: "_abi.SnnConn", ns: int, nt: int, device: torch.device, wmin: torch.Tensor, wmax: torch.Tensor,
+                         nu: Optional[torch.Tensor], owner=None) -> None:
+    """The per-synapse fields of a dense connection's plan entry (include/snn_b200.h): each bound that is a tensor of
+    more than one element, and ``nu`` (``torch.stack`` of the rule's two rates) when its rates are tensors; ``d.rule``
+    is set already.  The scalar fields of a tensor are left as the kernels ignore them, except the rates' gates."""
+    for name, t in (("wmin", wmin), ("wmax", wmax), ("nu", nu)):
+        if t is not None and t.numel() != 1 and t.device != device:   # the reference's first update fails on it
+            raise RuntimeError(f"Expected all tensors to be on the same device, but found at least two devices, {device} and "
+                               f"{t.device}! ({name} is on {t.device}, the weights on {device})")
+    if d.rule == _abi.SNN_RULE_WDEP_POSTPRE:
+        # WeightDependentPostPre multiplies every synapse's term by (w - wmin) / (wmax - w), including the zero terms of
+        # silent synapses (learning.py:640-649): an infinite bound turns them into NaN.  With scalar bounds the rule's
+        # constructor asserts finite ones; an infinite element of a bound tensor is refused here
+        gates = (d.nu0 != 0.0, d.nu1 != 0.0) if nu is None else (nu_any(nu, 0), nu_any(nu, 1))
+        for gate, t, name in ((gates[0], wmin, "wmin"), (gates[1], wmax, "wmax")):
+            if gate and _tensor_flag(t, "inf", lambda v: torch.isinf(v).any()):
+                raise NotImplementedError(f"WeightDependentPostPre with an infinite element of {name}: the reference's update turns "
+                                          "every weight of such a synapse into NaN (learning.py:640-649); use finite bounds")
+    for name, t, ptr, form in (("wmin", wmin, "wmin_t", "wmin_form"), ("wmax", wmax, "wmax_t", "wmax_form")):
+        if t.numel() != 1:
+            v, f = synapse_tensor(t, ns, nt, device, name, owner)
+            setattr(d, ptr, v.data_ptr())
+            setattr(d, form, f)
+    if nu is None:
+        return
+    pair = (nu[0], nu[1])
+    gates = [nu_any(nu, 0), nu_any(nu, 1)]
+    if d.rule == _abi.SNN_RULE_POSTPRE:
+        # PostPre scales the target traces / spikes by nu before torch.bmm (learning.py:403-417): a rate that does not
+        # broadcast to [1, n_tgt] makes the bmm fail once its term runs
+        for k, r in enumerate(pair):
+            if gates[k] and (r.dim() > 2 or (r.dim() == 2 and r.shape[0] != 1) or (r.dim() >= 1 and r.shape[-1] not in (1, nt))):
+                raise RuntimeError(f"PostPre: nu[{k}] of shape {list(r.shape)} does not broadcast to [1, {nt}]: torch.bmm fails on "
+                                   f"it (Expected size for first two dimensions of batch2 tensor to be: [B, 1] but got: [B, {ns}])")
+    if d.rule == _abi.SNN_RULE_HEBBIAN:
+        gates = [True, True]   # learning.py:1124-1134 applies both rates without a gate
+    if d.rule in (_abi.SNN_RULE_POSTPRE, _abi.SNN_RULE_WDEP_POSTPRE) and not any(gates):
+        d.nu0 = d.nu1 = 0.0    # neither term runs: nothing to read
+        return
+    v0, f0 = synapse_tensor(pair[0], ns, nt, device, "nu[0]", owner)
+    v1, f1 = synapse_tensor(pair[1], ns, nt, device, "nu[1]", owner)
+    d.nu0_t, d.nu0_form, d.nu1_t, d.nu1_form = v0.data_ptr(), f0, v1.data_ptr(), f1
+    d.nu0, d.nu1 = float(gates[0]), float(gates[1])
+
+
 class AbstractConnection(ABC, Module):
     """Reference: topology.py:17-156."""
 
@@ -122,19 +227,29 @@ class Connection(AbstractConnection):
 
             _plan.normalize_single_connection(self)
 
+    # per-synapse wmin / wmax and learning-rate tensors run on the generic kernel (LocalConnection and SparseConnection
+    # keep scalars)
+    _synapse_tensors = True
+
     # -- plan export -----------------------------------------------------------------------
     def _fill_desc(self, d: "_abi.SnnConn", dt: float, rule: bool = True) -> None:
         d.kind = _abi.SNN_CONN_DENSE
-        if self.wmin.numel() != 1 or self.wmax.numel() != 1:
-            raise NotImplementedError("per-synapse wmin/wmax tensors are not supported by the CUDA core yet")
-        d.wmin = _scalar(self.wmin, "wmin")
-        d.wmax = _scalar(self.wmax, "wmax")
+        tensors = self.wmin.numel() != 1 or self.wmax.numel() != 1
+        if tensors and not self._synapse_tensors:
+            raise NotImplementedError(f"per-synapse wmin/wmax tensors are not supported by the CUDA core on a {type(self).__name__}")
+        d.wmin = _scalar(self.wmin, "wmin") if self.wmin.numel() == 1 else -np.inf
+        d.wmax = _scalar(self.wmax, "wmax") if self.wmax.numel() == 1 else np.inf
         d.has_norm = int(self.norm is not None)
         d.norm_abs = 1
         d.norm = float(self.norm) if self.norm is not None else 0.0
         d.dt_scale = 1.0
         if rule:
             self.update_rule._fill_desc(d)
+            nu = self.update_rule.nu if getattr(self.update_rule, "_nu_tensors", False) else None
+            if tensors or nu is not None:
+                fill_synapse_tensors(d, self.source.n, self.target.n, self.w.device, self.wmin, self.wmax, nu, owner=self)
+                if nu is not None and d.rule == _abi.SNN_RULE_MSTDPET:
+                    d.dt_scale = float(getattr(self, "dt", dt))   # the kernel scales each rate: ((nu * dt) * reward) * e_trace
 
 
 def _pair(x):
@@ -549,6 +664,8 @@ class LocalConnection(Connection):
         if self.norm is not None:
             self.norm = self.norm * kernel_prod                                    # topology.py:1437-1438
 
+    _synapse_tensors = False
+
     def update(self, **kwargs) -> None:
         """topology.py:1457-1469."""
         if kwargs.get("mask", None) is None:
@@ -614,6 +731,8 @@ class SparseConnection(Connection):
         else:
             super().__init__(source, target, nu, reduction, weight_decay, w_dtype, **kwargs)
             self.w = Parameter(self.w.to_sparse(), requires_grad=False)          # topology.py:2017
+
+    _synapse_tensors = False
 
     def update(self, **kwargs) -> None:
         """topology.py:112-139 with the reference's refusal of masks on a sparse w (:129-131)."""

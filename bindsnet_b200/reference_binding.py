@@ -239,17 +239,31 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
             m = _u8(conn.mask.to(w.device)).contiguous()
             keep.append(m)
             d.mask = m.data_ptr()
-        d.wmin, d.wmax = _f(conn.wmin), _f(conn.wmax)
+        # wmin / wmax: scalars or tensors broadcasting to w (topology.py:74-81); the rule's nu: a pair of scalars or of
+        # tensors (learning.py:58-67)
+        tensors = conn.wmin.numel() != 1 or conn.wmax.numel() != 1 or rule.nu.dim() > 1
+        if tensors and type(conn).__name__ != "Connection":
+            raise NotImplementedError(f"per-synapse wmin / wmax or learning-rate tensors on a {type(conn).__name__}")
+        d.wmin = _f(conn.wmin) if conn.wmin.numel() == 1 else -math.inf
+        d.wmax = _f(conn.wmax) if conn.wmax.numel() == 1 else math.inf
         name = type(rule).__name__
         d.rule = {"NoOp": _abi.SNN_RULE_NOOP, "PostPre": _abi.SNN_RULE_POSTPRE, "Hebbian": _abi.SNN_RULE_HEBBIAN,
                   "WeightDependentPostPre": _abi.SNN_RULE_WDEP_POSTPRE}.get(name, -1)
         if d.rule < 0:
             raise NotImplementedError(f"learning rule {name}")
-        d.nu0, d.nu1 = _f(rule.nu[0]), _f(rule.nu[1])
+        if rule.nu.dim() == 1:
+            d.nu0, d.nu1 = _f(rule.nu[0]), _f(rule.nu[1])
         d.reduction = _reduction_code(rule.reduction)
         d.weight_decay = _f(rule.weight_decay)                                            # learning.py:85
-        finite = math.isfinite(d.wmin) or math.isfinite(d.wmax)
-        d.has_clamp = int(finite and name != "NoOp")                                      # learning.py:97-104
+        from .network.topology import bounds_clamp, fill_synapse_tensors
+
+        d.has_clamp = int(bounds_clamp(conn.wmin, conn.wmax) and name != "NoOp")          # learning.py:97-104
+        if tensors:
+            # the tensors the plan points at are kept alive with the plan (a copy only for a non-contiguous full layout)
+            owner = type("_Keep", (), {})()
+            fill_synapse_tensors(d, int(conn.source.n), int(conn.target.n), conn.w.device, conn.wmin.detach(), conn.wmax.detach(),
+                                 rule.nu if rule.nu.dim() > 1 else None, owner=owner)
+            keep.append(owner)
         if conn.b is not None:
             d.b = conn.b.data_ptr()
         if w.is_sparse:

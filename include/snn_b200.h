@@ -136,6 +136,13 @@ extern "C" {
 #define SNN_RULE_IS_MSTDP(r) ((r) == SNN_RULE_MSTDP || (r) == SNN_RULE_MSTDPET)
 #define SNN_RULE_IS_STDP(r) (((r) >= SNN_RULE_POSTPRE && (r) <= SNN_RULE_MCC_POSTPRE) || (r) == SNN_RULE_HEBBIAN)
 
+/* ---- broadcast forms of a dense connection's per-synapse tensors (snn_conn_t wmin_t / wmax_t / nu0_t / nu1_t): which
+ *      element (i, j) of [n_src, n_tgt] reads ---- */
+#define SNN_SYN_FULL 1 /* [n_src, n_tgt] row-major: t[i * n_tgt + j] */
+#define SNN_SYN_TGT 2  /* per target neuron, [n_tgt] (or [1, n_tgt]): t[j] */
+#define SNN_SYN_SRC 3  /* per source neuron, [n_src, 1]: t[i] */
+#define SNN_SYN_ONE 4  /* one element: t[0] */
+
 /* ---- weight-matrix structure hints (DiehlAndCook2015's static exc/inh matrices,
  *      models.py:204,217-220) ---- */
 #define SNN_W_DENSE 0   /* arbitrary dense matrix                                              */
@@ -278,10 +285,36 @@ typedef struct snn_conn {
        (torch.bernoulli(value) broadcast over B, topology_features.py:425-429).  The window draws with (opts.seed,
        opts.step_offset + t, connection index); snn_b200_conn_compute with (draw_seed, draw_step, draw_conn).  Generic
        tier only, and not in a plan that also holds an SNN_CONN_SPARSE connection. */
-    const float *f_prob;    /* Probability.value, each in [0, 1]                    topology_features.py:365-464 */
-    const uint8_t *f_mask;  /* Mask.value, 0 / 1 bytes                              topology_features.py:467-549 */
-    const float *f_int;     /* Intensity.value                                      topology_features.py:724-769 */
-    uint32_t draw_seed, draw_step, draw_conn;
+    /* SNN_CONN_DENSE keeps its per-synapse tensors in the same storage (a connection is never both kinds): wmin_t / wmax_t
+       are AbstractConnection.wmin / wmax (topology.py:74-81) and nu0_t / nu1_t the rows of LearningRule.nu =
+       torch.stack(nu) (learning.py:58-67), each float32 in the broadcast form its *_form byte names (SNN_SYN_*).  NULL
+       = the scalar field (wmin, wmax, nu0, nu1) holds the value.  nu0_t and nu1_t are set together.  Where a tensor is
+       set, the element (i, j) takes the scalar's place in every formula of the connection's rule:
+         clamp           w = clamp(w, wmin[i,j], wmax[i,j])  every step, for every rule but NOOP (has_clamp as for scalars:
+                         some element of wmin is not -inf, or some element of wmax is not +inf; learning.py:97-104)
+         POSTPRE         nu broadcast to [1, n_tgt] only (SNN_SYN_TGT / SNN_SYN_ONE; any other form is the reference's
+                         bmm shape error, SNN_ERR_BAD_ARG): U sums s_src * fl(x_tgt * nu0[j]), V sums x_src * nu1[j]
+         WDEP_POSTPRE    upd = 0 - fl(fl(nu0[i,j] * U) * (w - wmin[i,j])) + fl(fl(nu1[i,j] * V) * (wmax[i,j] - w))
+         HEBBIAN         w = w + nu0[i,j] * U;  w = w + nu1[i,j] * V
+         MSTDP           w = w + nu0[i,j] * upd
+         MSTDPET         w = w + fl(fl(fl(nu0[i,j] * dt_scale) * reward) * e_trace), dt_scale = connection.dt (et_coef unused)
+       With nu tensors the scalars nu0 / nu1 are the rule's gates: 0 when nu[k].any() is false, otherwise any non-zero
+       value (HEBBIAN applies its rates without a gate: nu0 = nu1 = 1).  Generic tier only (tier 0 selects it, a forced tier
+       2 or 3 is SNN_ERR_UNSUPPORTED), and not in a plan that also holds an SNN_CONN_SPARSE connection, MCC features or a
+       kind of the pooling instantiation.  A library older than these fields refuses such a plan (wmin_t, wmax_t and
+       nu0_t overlay f_prob / f_mask / f_int, which it accepts on SNN_CONN_MCC only). */
+    union {
+        struct {
+            const float *f_prob;    /* Probability.value, each in [0, 1]                    topology_features.py:365-464 */
+            const uint8_t *f_mask;  /* Mask.value, 0 / 1 bytes                              topology_features.py:467-549 */
+            const float *f_int;     /* Intensity.value                                      topology_features.py:724-769 */
+            uint32_t draw_seed, draw_step, draw_conn;
+        };
+        struct {
+            const float *wmin_t, *wmax_t, *nu0_t, *nu1_t;
+            int8_t wmin_form, wmax_form, nu0_form, nu1_form;
+        };
+    };
     /* SNN_CONN_MAXPOOL2D (topology.py:1124-1211): the firing_rates buffer [B, C, hin, win], updated in place (after a
        window it holds what the reference's buffer holds after the window's last compute), and the decay kwarg rounded
        to fp32 as `decay * firing_rates` rounds it. */

@@ -22,6 +22,10 @@ SNN_REDUCE_SUM, SNN_REDUCE_MEAN = 0, 1
 SNN_EXT_NONE, SNN_EXT_U8, SNN_EXT_F32 = 0, 1, 2
 SNN_W_DENSE, SNN_W_DIAG, SNN_W_OFFDIAG = 0, 1, 2
 SNN_SYN_FULL, SNN_SYN_TGT, SNN_SYN_SRC, SNN_SYN_ONE = 1, 2, 3, 4
+SNN_NODE_PN = 0x100
+(SNN_PN_THRESH, SNN_PN_REST, SNN_PN_DECAY, SNN_PN_THETA_PLUS, SNN_PN_THETA_DECAY, SNN_PN_TRACE_DECAY,
+ SNN_PN_TRACE_SCALE) = range(7)
+SNN_PN_ROWS = 7
 
 SNN_OK = 0
 SNN_ERR_BAD_ARG = 1
@@ -47,7 +51,23 @@ def describe_error(code: int) -> str:
     return ", ".join(name for bit, name in ERR_NAMES.items() if code & bit) or f"status {code}"
 
 
+class _CurrentFields(C.Structure):
+    _fields_ = [("i", C.c_void_p), ("i_decay", C.c_float)]
+
+
+class _NeuronParamFields(C.Structure):
+    _fields_ = [("pn", C.c_void_p), ("pn_mask", C.c_uint32)]
+
+
+class _CurrentOrNeuronParams(C.Union):
+    """The storage SNN_NODE_CURRENT_LIF's current and an SNN_NODE_PN layer's per-neuron block share."""
+
+    _anonymous_ = ("_cur", "_pn")
+    _fields_ = [("_cur", _CurrentFields), ("_pn", _NeuronParamFields)]
+
+
 class SnnLayer(C.Structure):
+    _anonymous_ = ("_u",)
     _fields_ = [
         ("kind", C.c_int32),
         ("n", C.c_int32),
@@ -85,8 +105,7 @@ class SnnLayer(C.Structure):
         ("rec_s", C.c_void_p),
         ("rec_v", C.c_void_p),
         ("rec_count", C.c_void_p),
-        ("i", C.c_void_p),
-        ("i_decay", C.c_float),
+        ("_u", _CurrentOrNeuronParams),
     ]
 
 

@@ -19,6 +19,40 @@ static thread_local int g_last_launches = 0;
 
 static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 
+// A LIF / DC layer's per-neuron block (snn_b200.h SNN_NODE_PN): a flag on those kinds only, a block wherever a row is
+// used, and rows only for the parameters the layer reads.
+static int pn_check(const snn_layer_t &L) {
+    const int kind = L.kind & ~SNN_NODE_PN;
+    if (kind != SNN_NODE_LIF && kind != SNN_NODE_DC) return SNN_ERR_BAD_ARG;
+    uint32_t allowed = 1u << SNN_PN_THRESH | 1u << SNN_PN_REST | 1u << SNN_PN_DECAY;
+    if (kind == SNN_NODE_DC) allowed |= 1u << SNN_PN_THETA_PLUS | 1u << SNN_PN_THETA_DECAY;
+    if (L.traces) allowed |= 1u << SNN_PN_TRACE_DECAY;
+    if (L.traces && L.traces_additive) allowed |= 1u << SNN_PN_TRACE_SCALE;
+    if ((L.pn_mask & ~allowed) || (L.pn_mask && !L.pn)) return SNN_ERR_BAD_ARG;
+    return SNN_OK;
+}
+
+// The plan every check and kernel below reads: the kinds without SNN_NODE_PN, pn_mask cleared on the LIF / DC layers
+// that do not carry the flag (their storage is CurrentLIFNodes' otherwise).  *pn: some layer uses a per-neuron row.
+static int strip_pn(const snn_net_t *net, snn_net_t *out, bool *pn) {
+    *pn = false;
+    if (!net || net->n_layers < 0 || net->n_layers > SNN_MAX_LAYERS) return SNN_ERR_BAD_ARG;
+    *out = *net;
+    for (int l = 0; l < net->n_layers; ++l) {
+        snn_layer_t &L = out->layers[l];
+        if (L.kind & SNN_NODE_PN) {
+            const int rc = pn_check(L);
+            if (rc != SNN_OK) return rc;
+            L.kind &= ~SNN_NODE_PN;
+            *pn |= L.pn_mask != 0u;
+        } else if (L.kind == SNN_NODE_LIF || L.kind == SNN_NODE_DC) {
+            L.pn = nullptr;
+            L.pn_mask = 0u;
+        }
+    }
+    return SNN_OK;
+}
+
 static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
     if (!net || !o || net->abi_version != SNN_ABI_VERSION) return SNN_ERR_BAD_ARG;
     if (net->n_layers < 1 || net->n_layers > SNN_MAX_LAYERS) return SNN_ERR_BAD_ARG;
@@ -230,12 +264,18 @@ const char *snn_b200_build_info(void) {
 
 int snn_b200_last_launch_count(void) { return g_last_launches; }
 
-int snn_b200_select_tier(const snn_net_t *net, const snn_run_opts_t *opts) {
+// (net: the plan strip_pn left; pn: some layer carries per-neuron parameters)
+static int select_tier(const snn_net_t *net, const snn_run_opts_t *opts, bool pn) {
     if (validate(net, opts) != SNN_OK) return 0;
     // one extra instantiation of the generic kernel each for sparse, feature and pooling plans (pooling: also plans with
     // a LocalConnection2D, a Conv3dConnection, SubtractiveResetIFNodes or PassThroughNodes), not combinations
     // (and one for plans with per-synapse bounds or rates)
     if ((int)has_sparse(net) + (int)has_feat(net) + (int)has_pool(net) + (int)has_syn(net) > 1) return 0;
+    // per-neuron parameters: two more instantiations, alone or with per-synapse tensors; the fused kernels read scalars
+    if (pn) {
+        if (has_sparse(net) || has_feat(net) || has_pool(net)) return 0;
+        return (opts->tier == 0 || opts->tier == 1) && !opts->delta_w && !opts->delta_theta ? 1 : 0;
+    }
     // the fused DiehlAndCook2015 kernels (and so the delta windows) have neither the sparse, the feature nor the pooling
     // gather, and read scalar bounds and rates only
     if (has_sparse(net) || has_feat(net) || has_pool(net) || has_syn(net))
@@ -252,24 +292,40 @@ int snn_b200_select_tier(const snn_net_t *net, const snn_run_opts_t *opts) {
     return 1;
 }
 
-size_t snn_b200_workspace_bytes(const snn_net_t *net, const snn_run_opts_t *opts) {
+int snn_b200_select_tier(const snn_net_t *net, const snn_run_opts_t *opts) {
+    snn_net_t P;
+    bool pn;
+    if (strip_pn(net, &P, &pn) != SNN_OK) return 0;
+    return select_tier(&P, opts, pn);
+}
+
+size_t snn_b200_workspace_bytes(const snn_net_t *net0, const snn_run_opts_t *opts) {
+    snn_net_t P;
+    bool pn;
+    if (strip_pn(net0, &P, &pn) != SNN_OK) return 0;
+    const snn_net_t *net = &P;
     if (validate(net, opts) != SNN_OK) return 0;
     size_t g = layout_generic(net, opts, nullptr, nullptr);
-    if (has_sparse(net) || has_feat(net) || has_pool(net) || has_syn(net)) return g;
+    if (pn || has_sparse(net) || has_feat(net) || has_pool(net) || has_syn(net)) return g;
     size_t f = snn_fused_dc_supported(net, opts) ? snn_fused_dc_workspace_bytes(net, opts) : 0;
     size_t f2 = snn_fused_dc2_supported(net, opts) ? snn_fused_dc2_workspace_bytes(net, opts) : 0;
     if (f2 > f) f = f2;
     return g > f ? g : f;
 }
 
-int snn_b200_run_window(const snn_net_t *net, const snn_run_opts_t *opts, void *workspace, size_t workspace_bytes,
+int snn_b200_run_window(const snn_net_t *net0, const snn_run_opts_t *opts, void *workspace, size_t workspace_bytes,
                         void *stream_) {
     g_last_launches = 0;
-    int rc = validate(net, opts);
+    snn_net_t P;
+    bool pn;
+    int rc = strip_pn(net0, &P, &pn);
+    if (rc != SNN_OK) return rc;
+    const snn_net_t *net = &P;
+    rc = validate(net, opts);
     if (rc != SNN_OK) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     if (opts->T == 0 && !opts->normalize) return SNN_OK;
-    const int tier = snn_b200_select_tier(net, opts);
+    const int tier = select_tier(net, opts, pn);
     if (tier == 0) return SNN_ERR_UNSUPPORTED;
     if (!workspace) return SNN_ERR_WORKSPACE;
     if (tier == 3) {

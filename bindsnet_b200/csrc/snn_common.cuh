@@ -265,16 +265,45 @@ __device__ __forceinline__ float trace_step(float x, bool s, float decay, float 
     return x;
 }
 
-// LIFNodes.forward (nodes.py:500-529).  `xin` is masked in place like the reference does.
-__device__ __forceinline__ bool lif_step(const snn_layer_t &L, float &v, float &rc, float &xin) {
-    v = L.decay * (v - L.rest) + L.rest;
+// The parameters a neuron of an SNN_NODE_LIF / SNN_NODE_DC layer reads (snn_b200.h SNN_NODE_PN): the layer's scalars, or
+// the neuron's row of the per-neuron block where pn_mask has the bit.
+struct NeuronPar {
+    float thresh, rest, decay, theta_plus, theta_decay, trace_decay, trace_scale;
+};
+// pn_mask of a layer whose storage holds a per-neuron block (the library zeroes it on LIF / DC layers without the flag)
+__device__ __forceinline__ uint32_t pn_mask_of(const snn_layer_t &L) {
+    return L.kind == SNN_NODE_LIF || L.kind == SNN_NODE_DC ? L.pn_mask : 0u;
+}
+__device__ __forceinline__ float pn_at(const snn_layer_t &L, uint32_t mask, int row, float scalar, int j) {
+    return (mask >> row) & 1u ? __ldg(L.pn + (size_t)row * L.n + j) : scalar;
+}
+__device__ __forceinline__ NeuronPar neuron_par(const snn_layer_t &L, int j) {
+    const uint32_t m = pn_mask_of(L);
+    NeuronPar P;
+    P.thresh = pn_at(L, m, SNN_PN_THRESH, L.thresh, j);
+    P.rest = pn_at(L, m, SNN_PN_REST, L.rest, j);
+    P.decay = pn_at(L, m, SNN_PN_DECAY, L.decay, j);
+    P.theta_plus = pn_at(L, m, SNN_PN_THETA_PLUS, L.theta_plus, j);
+    P.theta_decay = pn_at(L, m, SNN_PN_THETA_DECAY, L.theta_decay, j);
+    P.trace_decay = pn_at(L, m, SNN_PN_TRACE_DECAY, L.trace_decay, j);
+    P.trace_scale = pn_at(L, m, SNN_PN_TRACE_SCALE, L.trace_scale, j);
+    return P;
+}
+
+// LIFNodes.forward (nodes.py:500-529) with the neuron's decay, rest and threshold.  `xin` is masked in place like the
+// reference does.
+__device__ __forceinline__ bool lif_step_p(const snn_layer_t &L, float decay, float rest, float thresh, float &v, float &rc, float &xin) {
+    v = decay * (v - rest) + rest;
     if (rc > 0.0f) xin = 0.0f;
     rc = rc - L.dt;
     v = v + xin;
-    const bool s = v >= L.thresh;
+    const bool s = v >= thresh;
     if (s) { rc = L.refrac; v = L.reset; }
     if (L.has_lbound && v < L.lbound) v = L.lbound;
     return s;
+}
+__device__ __forceinline__ bool lif_step(const snn_layer_t &L, float &v, float &rc, float &xin) {
+    return lif_step_p(L, L.decay, L.rest, L.thresh, v, rc, xin);
 }
 
 // IFNodes.forward (nodes.py:377-394): no leak, the gate is taken before the refractory decrement, x stays unmasked.
@@ -335,15 +364,20 @@ __device__ __forceinline__ bool boosted_step(const snn_layer_t &L, float &v, flo
 }
 
 // DiehlAndCookNodes.forward up to the threshold test (nodes.py:1077-1092); `theta` is the
-// already decayed adaptive threshold of the neuron.  Returns the candidate flag.
-__device__ __forceinline__ bool dc_step(const snn_layer_t &L, float &v, float &rc, float xin, float theta) {
-    v = L.decay * (v - L.rest) + L.rest;
+// already decayed adaptive threshold of the neuron.  Returns the candidate flag.  dc_step_p: with the neuron's decay,
+// rest and threshold.
+__device__ __forceinline__ bool dc_step_p(const snn_layer_t &L, float decay, float rest, float thresh, float &v, float &rc, float xin,
+                                          float theta) {
+    v = decay * (v - rest) + rest;
     const float gate = rc <= 0.0f ? 1.0f : 0.0f;
     v = v + gate * xin;
     rc = rc - L.dt;
-    const bool s = v >= (L.thresh + theta);
+    const bool s = v >= (thresh + theta);
     if (s) { rc = L.refrac; v = L.reset; }
     return s;
+}
+__device__ __forceinline__ bool dc_step(const snn_layer_t &L, float &v, float &rc, float xin, float theta) {
+    return dc_step_p(L, L.decay, L.rest, L.thresh, v, rc, xin, theta);
 }
 
 // One STDP-family update of a single synapse, in the reference's order: pre term, post term,

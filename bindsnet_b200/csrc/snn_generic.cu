@@ -63,7 +63,9 @@ __device__ __forceinline__ void sparse_unit(const DevNet &N, int u, int &c, int 
 // step (or, in one-step mode, before the barrier that ends the source layer).
 // SYN: some dense connection carries per-synapse bounds or rates (snn_b200.h); only the learning phase differs, and
 // plans without them run the instantiation whose code never reads those fields.  Not combined with SPARSE, FEAT or POOL.
-template <int CTAS, bool SPARSE, bool FEAT, bool POOL, bool SYN = false>
+// PN: some LIF / DC layer carries per-neuron parameters (snn_b200.h SNN_NODE_PN); phases 1 and 2 and the theta of the
+// last step read a lane's own values where the other instantiations read the layer's scalars.  Combined with SYN only.
+template <int CTAS, bool SPARSE, bool FEAT, bool POOL, bool SYN = false, bool PN = false>
 __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(const __grid_constant__ DevNet N) {
 #ifdef SNN_EMU
     float *smem = emu::tls_cta->dyn_smem;
@@ -145,10 +147,10 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                     for (int c = 0; c < N.n_conns; ++c) any |= N.conns[c].kind == SNN_CONN_SPARSE && N.conns[c].tgt == l;
                     if (any && !grid_barrier(N.bar, G, N.err, bgen)) return;
                 }
-                for (int u = blockIdx.x; u < D.nw * nch; u += G) phase1<SPARSE, FEAT, POOL>(N, l, u / nch, u % nch, t, M);
+                for (int u = blockIdx.x; u < D.nw * nch; u += G) phase1<SPARSE, FEAT, POOL, PN>(N, l, u / nch, u % nch, t, M);
                 if (D.L.kind == SNN_NODE_DC && D.L.one_spike) {
                     if (!grid_barrier(N.bar, G, N.err, bgen)) return;
-                    for (int u = blockIdx.x; u < D.nw * nch; u += G) phase2<POOL>(N, l, u / nch, u % nch, t);
+                    for (int u = blockIdx.x; u < D.nw * nch; u += G) phase2<POOL, PN>(N, l, u / nch, u % nch, t);
                 }
                 if (l + 1 < N.n_layers && !grid_barrier(N.bar, G, N.err, bgen)) return;
             }
@@ -164,7 +166,7 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
             }
             for (int u = blockIdx.x; u < N.total_items * nch; u += G) {
                 int li, tile; item_of(N, u / nch, li, tile);
-                phase1<SPARSE, FEAT, POOL>(N, li, tile, u % nch, t, M);
+                phase1<SPARSE, FEAT, POOL, PN>(N, li, tile, u % nch, t, M);
             }
         }
         GPROF(0)
@@ -174,7 +176,7 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
             for (int u = blockIdx.x; u < N.total_items * nch; u += G) {
                 int li, tile; item_of(N, u / nch, li, tile);
                 const snn_layer_t &L = N.layers[li].L;
-                if (L.kind == SNN_NODE_DC && L.one_spike) phase2<POOL>(N, li, tile, u % nch, t);
+                if (L.kind == SNN_NODE_DC && L.one_spike) phase2<POOL, PN>(N, li, tile, u % nch, t);
             }
             GPROF(2)
         }
@@ -230,7 +232,8 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
             const int j = tile * SNN_TILE + lane;
             if (D.thcnt && D.L.learning && warp == 0 && j < D.L.n) {
                 const int tl = N.T - 1;
-                D.L.theta[j] = __ldcg(D.thdec + (size_t)(tl & 1) * D.L.n + j) + D.L.theta_plus * (float)__ldcg(D.thcnt + (size_t)(tl % 3) * D.L.n + j);
+                const float tplus = PN ? pn_at(D.L, pn_mask_of(D.L), SNN_PN_THETA_PLUS, D.L.theta_plus, j) : D.L.theta_plus;
+                D.L.theta[j] = __ldcg(D.thdec + (size_t)(tl & 1) * D.L.n + j) + tplus * (float)__ldcg(D.thcnt + (size_t)(tl % 3) * D.L.n + j);
             }
         }
     if (N.normalize) {
@@ -252,6 +255,15 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
 }  // namespace
 
 size_t snn_generic_smem_bytes(int B) { return gen_smem_bytes(B); }
+
+// some LIF / DC layer of the plan carries per-neuron parameters (the library keeps pn_mask zero on every other one)
+static bool snn_dev_has_pn(const DevNet &N) {
+    for (int l = 0; l < N.n_layers; ++l) {
+        const snn_layer_t &L = N.layers[l].L;
+        if ((L.kind == SNN_NODE_LIF || L.kind == SNN_NODE_DC) && L.pn_mask) return true;
+    }
+    return false;
+}
 
 // The work decomposition (sample chunks of phases 1 / 2, learning-phase units) for a grid of at most `cap` co-resident
 // CTAs; returns the grid size.
@@ -310,6 +322,10 @@ int snn_generic_launch(DevNet &N, cudaStream_t) {
     if (N.sp_units) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, true, false, false>(*(const DevNet *)a); }, &N);
     else if (N.any_feat) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, true, false>(*(const DevNet *)a); }, &N);
     else if (N.any_pool) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, true>(*(const DevNet *)a); }, &N);
+    else if (snn_dev_has_pn(N) && std::any_of(N.conns, N.conns + N.n_conns, snn_has_syn))
+        emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, false, true, true>(*(const DevNet *)a); }, &N);
+    else if (snn_dev_has_pn(N))
+        emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, false, false, true>(*(const DevNet *)a); }, &N);
     else if (std::any_of(N.conns, N.conns + N.n_conns, snn_has_syn))
         emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, false, true>(*(const DevNet *)a); }, &N);
     else emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, false>(*(const DevNet *)a); }, &N);
@@ -328,10 +344,13 @@ int snn_generic_launch(DevNet &N, cudaStream_t stream) {
     // MCC features or the POOL instantiation's kinds)
     const bool sparse = std::any_of(N.conns, N.conns + N.n_conns, [](const snn_conn_t &C) { return C.kind == SNN_CONN_SPARSE; });
     const bool syn = std::any_of(N.conns, N.conns + N.n_conns, snn_has_syn);
+    const bool pn = snn_dev_has_pn(N);
     bool three = false;
-    if (const char *v = getenv("SNN_B200_GVAR")) three = !sparse && !N.any_feat && !N.any_pool && !syn && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
+    if (const char *v = getenv("SNN_B200_GVAR")) three = !sparse && !N.any_feat && !N.any_pool && !syn && !pn && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
     const void *kern = three ? (const void *)snn_generic_window<3, false, false, false>
                      : sparse ? (const void *)snn_generic_window<2, true, false, false>
+                     : pn ? (syn ? (const void *)snn_generic_window<2, false, false, false, true, true>
+                               : (const void *)snn_generic_window<2, false, false, false, false, true>)
                      : syn ? (const void *)snn_generic_window<2, false, false, false, true>
                      : N.any_feat ? (const void *)snn_generic_window<2, false, true, false>
                      : N.any_pool ? (const void *)snn_generic_window<2, false, false, true> : (const void *)snn_generic_window<2, false, false, false>;

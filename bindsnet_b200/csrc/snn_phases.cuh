@@ -490,14 +490,16 @@ __device__ __forceinline__ int pool_argmax(const snn_conn_t &C, const float *r, 
 // Final spikes of one neuron of one sample: traces (nodes.py:96-103), clamp / unclamp (network.py:415-429),
 // recordings, and (POOL) the next rate of every MaxPool2dConnection leaving the layer.  Returns the spike that is published.
 // (POOL) A PassThroughNodes layer has no traces (its forward never reaches Nodes.forward) and a float32 s.
-template <bool POOL>
+// (PN) `P` holds the neuron's trace decay and scale (snn_b200.h SNN_NODE_PN).
+template <bool POOL, bool PN = false>
 __device__ __forceinline__ bool finalize_neuron(const DevNet &N, const DevLayer &D, bool s, float xold, size_t k, int b, int j, int t, int wr,
-                                                int li) {
+                                                int li, const NeuronPar *P = nullptr) {
     const snn_layer_t &L = D.L;
     const bool pass = POOL && L.kind == SNN_NODE_PASSTHROUGH;
     bool sf = s;
     if (L.traces && !pass) {
-        const float x = trace_step(xold, s, L.trace_decay, L.trace_scale, L.traces_additive);
+        const float x = PN ? trace_step(xold, s, P->trace_decay, P->trace_scale, L.traces_additive)
+                           : trace_step(xold, s, L.trace_decay, L.trace_scale, L.traces_additive);
         L.x[k] = x;
         if (D.xpub) D.xpub[((size_t)wr * N.B + b) * L.n + j] = x;
     }
@@ -516,7 +518,8 @@ __device__ __forceinline__ bool finalize_neuron(const DevNet &N, const DevLayer 
 // ---------------------------------------------------------------------------------------
 // phase 1.  Work unit = (layer, 32-neuron tile, chunk of N.cs samples): one warp lane per neuron, the CTA's
 // warps stride over the chunk's samples.
-template <bool SPARSE, bool FEAT, bool POOL>
+// PN: some layer carries per-neuron parameters (snn_b200.h SNN_NODE_PN); a lane loads its neuron's once per unit.
+template <bool SPARSE, bool FEAT, bool POOL, bool PN = false>
 __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, const GenSmem &M) {
     const DevLayer &D = N.layers[li];
     const snn_layer_t &L = D.L;
@@ -569,12 +572,15 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
     // integer accumulated with atomics over the sample chunks (thcnt[t % 3]); every unit rebuilds the value the
     // previous step left — thdec (the decayed threshold that step used) + theta_plus * count — so no unit waits
     // for another one; chunk 0 publishes this step's decayed value and clears the counter slot of step t + 1.
+    NeuronPar P;
+    if (PN) P = neuron_par(L, valid ? j : 0);
     float theta = 0.0f;
     if (dc && valid) {
         if (L.learning) {
+            const float tplus = PN ? P.theta_plus : L.theta_plus;
             const float prev = t == 0 ? L.theta[j]
-                                      : __ldcg(D.thdec + (size_t)rd * n + j) + L.theta_plus * (float)__ldcg(D.thcnt + (size_t)((t + 2) % 3) * n + j);
-            theta = prev * L.theta_decay;
+                                      : __ldcg(D.thdec + (size_t)rd * n + j) + tplus * (float)__ldcg(D.thcnt + (size_t)((t + 2) % 3) * n + j);
+            theta = prev * (PN ? P.theta_decay : L.theta_decay);
             if (chunk == 0 && warp == 0) {
                 D.thdec[(size_t)wr * n + j] = theta;
                 D.thcnt[(size_t)((t + 1) % 3) * n + j] = 0;
@@ -737,7 +743,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
                 s = xin != 0.0f;
                 nonbin |= s && xin != 1.0f;
             } else if (dc) {
-                s = dc_step(L, v, rc, xin, theta);
+                s = PN ? dc_step_p(L, P.decay, P.rest, P.thresh, v, rc, xin, theta) : dc_step(L, v, rc, xin, theta);
                 if (L.has_lbound && v < L.lbound) v = L.lbound;  // nodes.py:1108-1109
             } else if (L.kind == SNN_NODE_IF) {
                 s = if_step(L, v, rc, xin);
@@ -752,7 +758,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
             } else if (POOL && L.kind == SNN_NODE_SUBIF) {
                 s = subif_step(L, v, rc, xin);
             } else {
-                s = lif_step(L, v, rc, xin);
+                s = PN ? lif_step_p(L, P.decay, P.rest, P.thresh, v, rc, xin) : lif_step(L, v, rc, xin);
             }
             if (!pass) {
                 L.v[k] = v;
@@ -777,7 +783,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
             }
         } else {
             bool sf = false;
-            if (valid) sf = finalize_neuron<POOL>(N, D, s, xold, k, b, j, t, wr, li);
+            if (valid) sf = finalize_neuron<POOL, PN>(N, D, s, xold, k, b, j, t, wr, li, &P);
             const uint32_t fw = __ballot_sync(0xffffffffu, valid && sf);
             if (lane == 0) {
                 D.bits[((size_t)wr * B + b) * nw + tile] = fw;
@@ -800,8 +806,8 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
 
 // ---------------------------------------------------------------------------------------
 // phase 2 (DiehlAndCookNodes with one_spike): keep the arg-max candidate of each sample
-// (nodes.py:1097-1105), then traces / clamp / publish as in phase 1.  Same work units as phase 1.
-template <bool POOL>
+// (nodes.py:1097-1105), then traces / clamp / publish as in phase 1.  Same work units as phase 1.  PN: as for phase 1.
+template <bool POOL, bool PN = false>
 __device__ void phase2(const DevNet &N, int li, int tile, int chunk, int t) {
     const DevLayer &D = N.layers[li];
     const snn_layer_t &L = D.L;
@@ -809,6 +815,8 @@ __device__ void phase2(const DevNet &N, int li, int tile, int chunk, int t) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int j = tile * SNN_TILE + lane;
     const bool valid = j < n;
+    NeuronPar P;
+    if (PN) P = neuron_par(L, valid ? j : 0);
     const int wr = t & 1;
     const int b0 = chunk * N.cs, b1 = min(B, b0 + N.cs);
     for (int bb = b0 + warp; bb < b1; bb += 4 * SNN_GEN_WARPS) {
@@ -830,7 +838,7 @@ __device__ void phase2(const DevNet &N, int li, int tile, int chunk, int t) {
             const size_t k = (size_t)b * n + j;
             const bool s = valid && ((cand[q] >> lane) & 1u) && key[q] != 0ull && (uint32_t)(key[q] & 0xffffffffull) == (uint32_t)j;
             bool sf = false;
-            if (valid) sf = finalize_neuron<POOL>(N, D, s, xo[q], k, b, j, t, wr, li);
+            if (valid) sf = finalize_neuron<POOL, PN>(N, D, s, xo[q], k, b, j, t, wr, li, &P);
             const uint32_t fw = __ballot_sync(0xffffffffu, valid && sf);
             if (lane == 0) {
                 D.bits[((size_t)wr * B + b) * nw + tile] = fw;

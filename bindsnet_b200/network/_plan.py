@@ -50,7 +50,7 @@ def fill_layer(d: "_abi.SnnLayer", layer, name: str, B: int) -> None:
         d.v = _ptr(_state(layer.v, "v", name))
         if d.kind != _abi.SNN_NODE_MCP:
             d.refrac_count = _ptr(_state(layer.refrac_count, "refrac_count", name))
-    if d.kind == _abi.SNN_NODE_DC:
+    if d.kind & ~_abi.SNN_NODE_PN == _abi.SNN_NODE_DC:   # (with or without per-neuron parameters)
         d.theta = _ptr(_state(layer.theta, "theta", name))
     if d.kind == _abi.SNN_NODE_CURRENT_LIF:
         d.i = _ptr(_state(layer.i, "i", name))
@@ -318,7 +318,23 @@ def build_net(
         raise NotImplementedError("a network with a MaxPool2dConnection, LocalConnection2D, Conv3dConnection, SubtractiveResetIFNodes or "
                                   "PassThroughNodes and a SparseConnection or MulticompartmentConnection features is not "
                                   "implemented by the CUDA core (each has its own instantiation of the window kernel)")
+    check_neuron_params(layers, conns)
     return net, keep
+
+
+def check_neuron_params(layers, conns) -> None:
+    """Per-neuron parameters (include/snn_b200.h SNN_NODE_PN) run on their own instantiations of the window kernel,
+    alone or with per-synapse bounds and rates: refuse, before anything runs, a plan that also needs the sparse, feature
+    or pooling one."""
+    if not any(d.kind & _abi.SNN_NODE_PN for d in layers):
+        return
+    pool_kinds = (_abi.SNN_CONN_MAXPOOL2D, _abi.SNN_CONN_LOCAL2D, _abi.SNN_CONN_CONV3D)
+    if any(d.kind == _abi.SNN_CONN_SPARSE or d.kind in pool_kinds or (d.kind == _abi.SNN_CONN_MCC and (d.f_prob or d.f_mask or d.f_int))
+           for d in conns) or any(d.kind in CONVERSION_KINDS for d in layers):
+        raise NotImplementedError("per-neuron parameter tensors in a network with a SparseConnection, MulticompartmentConnection "
+                                  "features, a MaxPool2dConnection, LocalConnection2D, Conv3dConnection, SubtractiveResetIFNodes "
+                                  "or PassThroughNodes are not implemented by the CUDA core (each has its own instantiation of "
+                                  "the window kernel)")
 
 
 CONVERSION_KINDS = (_abi.SNN_NODE_SUBIF, _abi.SNN_NODE_PASSTHROUGH)

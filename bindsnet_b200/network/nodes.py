@@ -51,6 +51,50 @@ def _scalar(value: Scalar, name: str) -> float:
     return float(value)
 
 
+def _per_neuron(value) -> bool:
+    """A parameter given as a tensor of more than one element (one element stays a scalar, whatever its shape)."""
+    return isinstance(value, torch.Tensor) and value.numel() != 1
+
+
+def _no_tensor_fill(value, name: str, op: str = "masked_fill_") -> None:
+    """The reference writes ``refrac`` / ``reset`` / ``lbound`` / a non-additive ``trace_scale`` with ``masked_fill_`` and
+    ``rest`` with ``fill_``, which take a 0-dim value only: its first step (or reset) raises this ``RuntimeError``."""
+    if _per_neuron(value):
+        if op == "fill_":
+            raise RuntimeError(f"fill_ only supports 0-dimension value tensor but got tensor with {value.dim()} dimensions. "
+                               f"('{name}' is a per-neuron tensor)")
+        raise RuntimeError(f"masked_fill_ only supports a 0-dimensional value tensor, but got tensor with {value.dim()} "
+                           f"dimension(s). ('{name}' is a per-neuron tensor)")
+
+
+_ROW_CACHE: dict = {}
+
+
+def _neuron_row(value: torch.Tensor, name: str, shape, device) -> torch.Tensor:
+    """A per-neuron parameter as ``[n]`` fp32 on ``device``, cached per tensor object and version like ``_scalar``.  It
+    must broadcast to the layer's shape without growing it (``[n]``, the full shape, or e.g. ``[C, 1, 1]`` of a
+    ``[C, H, W]`` layer): the reference broadcasts it elementwise against ``[B, *shape]``."""
+    shape = tuple(shape)
+    try:
+        out_shape = torch.broadcast_shapes(tuple(value.shape), shape)
+    except RuntimeError as e:
+        raise RuntimeError(f"per-neuron '{name}' of shape {tuple(value.shape)} does not broadcast to the layer's shape "
+                           f"{shape}: {e}") from None
+    if tuple(out_shape) != shape:
+        raise NotImplementedError(f"per-neuron '{name}' of shape {tuple(value.shape)} broadcasts the layer's state {shape} "
+                                  f"to {tuple(out_shape)}; the CUDA core keeps one value per neuron")
+    key = (id(value), str(device))
+    hit = _ROW_CACHE.get(key)
+    if hit is not None and hit[0] is value and hit[1] == value._version:
+        return hit[2]
+    with torch.no_grad():
+        row = value.detach().to(device, torch.float32).expand(shape).reshape(-1).contiguous()
+    if len(_ROW_CACHE) > 4096:
+        _ROW_CACHE.clear()
+    _ROW_CACHE[key] = (value, value._version, row)
+    return row
+
+
 class Nodes(torch.nn.Module):
     """Base class of all populations (reference: nodes.py:9-162)."""
 
@@ -153,7 +197,9 @@ class Nodes(torch.nn.Module):
         return super().train(mode)
 
     # -- plan export -----------------------------------------------------------------------
-    def _fill_desc(self, d: "_abi.SnnLayer") -> None:
+    def _fill_desc(self, d: "_abi.SnnLayer", rows: Optional[dict] = None) -> None:
+        """``rows``: collects the per-neuron parameters (``{SNN_PN_*: (name, tensor)}``) of a population that runs them
+        (``LIFNodes``, ``AdaptiveLIFNodes``, ``DiehlAndCookNodes``); without it a tensor parameter is refused."""
         if self.kind is None:
             raise NotImplementedError(
                 f"{type(self).__name__} has no CUDA implementation in bindsnet_b200 "
@@ -168,8 +214,36 @@ class Nodes(torch.nn.Module):
         d.learning = int(bool(self.learning))
         d.dt = float(self.dt) if self.dt is not None else 1.0
         if self.traces:
-            d.trace_decay = _scalar(self.trace_decay, "tc_trace")
-            d.trace_scale = _scalar(self.trace_scale, "trace_scale")
+            d.trace_decay = self._param(self.trace_decay, "tc_trace", _abi.SNN_PN_TRACE_DECAY, rows)
+            if rows is not None and not self.traces_additive:
+                _no_tensor_fill(self.trace_scale, "trace_scale")
+            d.trace_scale = self._param(self.trace_scale, "trace_scale", _abi.SNN_PN_TRACE_SCALE, rows)
+
+    @staticmethod
+    def _param(value, name: str, row: int, rows: Optional[dict]) -> float:
+        """The scalar field of a parameter; a per-neuron tensor goes to ``rows`` (its scalar field is then unused)."""
+        if rows is not None and _per_neuron(value):
+            rows[row] = (name, value)
+            return 0.0
+        return _scalar(value, name)
+
+    def _fill_rows(self, d: "_abi.SnnLayer", rows: dict) -> None:
+        """The per-neuron block of ``rows`` (include/snn_b200.h SNN_NODE_PN): ``[SNN_PN_ROWS, n]`` fp32 on the layer's
+        device, rebuilt only when one of its tensors changed."""
+        if not rows:
+            return
+        device = self.s.device
+        key = (tuple(sorted((r, id(t), t._version) for r, (_, t) in rows.items())), str(device), self.n)
+        cached = getattr(self, "_b200_pn", None)
+        if cached is None or cached[0] != key:
+            block = torch.zeros(_abi.SNN_PN_ROWS, self.n, dtype=torch.float32, device=device)
+            for r, (name, t) in rows.items():
+                block[r].copy_(_neuron_row(t, name, self.shape, device))
+            mask = sum(1 << r for r in rows)
+            cached = (key, block, mask, [t for _, t in rows.values()])
+            self._b200_pn = cached
+        d.kind = d.kind | _abi.SNN_NODE_PN
+        d.pn, d.pn_mask = cached[1].data_ptr(), cached[2]
 
 
 class AbstractInput:
@@ -236,11 +310,13 @@ class LIFNodes(Nodes):
 
     def reset_state_variables(self) -> None:
         """nodes.py:531-538."""
+        _no_tensor_fill(self.rest, "rest", "fill_")   # (raised before any state changes)
         super().reset_state_variables()
         self.v.fill_(self.rest)
         self.refrac_count.zero_()
 
     def _reset_plan(self):
+        _no_tensor_fill(self.rest, "rest", "fill_")
         zeros, fills = super()._reset_plan()
         return zeros + [self.refrac_count], fills + [(self.v, self.rest)]
 
@@ -257,14 +333,21 @@ class LIFNodes(Nodes):
         self.refrac_count = torch.zeros_like(self.v)
 
     def _fill_desc(self, d) -> None:
-        super()._fill_desc(d)
-        d.decay = _scalar(self.decay, "tc_decay")
-        d.rest = _scalar(self.rest, "rest")
+        # per-neuron thresh / rest / tc_decay / traces on LIFNodes itself (not on CurrentLIFNodes)
+        rows = {} if self.kind == _abi.SNN_NODE_LIF else None
+        if rows is not None:
+            for name in ("refrac", "reset", "lbound"):
+                _no_tensor_fill(getattr(self, name), name)
+        super()._fill_desc(d, rows)
+        d.decay = self._param(self.decay, "tc_decay", _abi.SNN_PN_DECAY, rows)
+        d.rest = self._param(self.rest, "rest", _abi.SNN_PN_REST, rows)
         d.reset = _scalar(self.reset, "reset")
-        d.thresh = _scalar(self.thresh, "thresh")
+        d.thresh = self._param(self.thresh, "thresh", _abi.SNN_PN_THRESH, rows)
         d.refrac = _scalar(self.refrac, "refrac")
         d.has_lbound = int(self.lbound is not None)
         d.lbound = _scalar(self.lbound, "lbound") if self.lbound is not None else 0.0
+        if rows is not None:
+            self._fill_rows(d, rows)
 
 
 class DiehlAndCookNodes(Nodes):
@@ -313,12 +396,14 @@ class DiehlAndCookNodes(Nodes):
         self.one_spike = one_spike
 
     def reset_state_variables(self) -> None:
-        """nodes.py:1113-1120 — ``theta`` is deliberately NOT reset."""
+        """nodes.py:1113-1120 (AdaptiveLIFNodes :948-955) — ``theta`` is deliberately NOT reset."""
+        _no_tensor_fill(self.rest, "rest", "fill_")   # (raised before any state changes)
         super().reset_state_variables()
         self.v.fill_(self.rest)
         self.refrac_count.zero_()
 
     def _reset_plan(self):
+        _no_tensor_fill(self.rest, "rest", "fill_")
         zeros, fills = super()._reset_plan()
         return zeros + [self.refrac_count], fills + [(self.v, self.rest)]
 
@@ -336,14 +421,18 @@ class DiehlAndCookNodes(Nodes):
         self.refrac_count = torch.zeros_like(self.v)
 
     def _fill_desc(self, d) -> None:
-        super()._fill_desc(d)
-        d.decay = _scalar(self.decay, "tc_decay")
-        d.rest = _scalar(self.rest, "rest")
+        rows = {}
+        for name in ("refrac", "reset", "lbound"):
+            _no_tensor_fill(getattr(self, name), name)
+        super()._fill_desc(d, rows)
+        d.decay = self._param(self.decay, "tc_decay", _abi.SNN_PN_DECAY, rows)
+        d.rest = self._param(self.rest, "rest", _abi.SNN_PN_REST, rows)
         d.reset = _scalar(self.reset, "reset")
-        d.thresh = _scalar(self.thresh, "thresh")
+        d.thresh = self._param(self.thresh, "thresh", _abi.SNN_PN_THRESH, rows)
         d.refrac = _scalar(self.refrac, "refrac")
-        d.theta_plus = _scalar(self.theta_plus, "theta_plus")
-        d.theta_decay = _scalar(self.theta_decay, "tc_theta_decay")
+        d.theta_plus = self._param(self.theta_plus, "theta_plus", _abi.SNN_PN_THETA_PLUS, rows)
+        d.theta_decay = self._param(self.theta_decay, "tc_theta_decay", _abi.SNN_PN_THETA_DECAY, rows)
+        self._fill_rows(d, rows)
         d.one_spike = int(bool(self.one_spike))
         d.has_lbound = int(self.lbound is not None)
         d.lbound = _scalar(self.lbound, "lbound") if self.lbound is not None else 0.0

@@ -55,8 +55,10 @@ def fill_layer(d: "_abi.SnnLayer", layer, B: int, keep: List[torch.Tensor]) -> N
     d.traces, d.traces_additive = int(layer.traces), int(layer.traces_additive)
     d.sum_input, d.learning = int(layer.sum_input), int(layer.learning)
     d.dt = _f(layer.dt)
+    rows = _neuron_rows(layer, kind)
+    _g = lambda name: 0.0 if name in rows else _f(getattr(layer, name))                # a per-neuron row replaces the scalar
     if layer.traces:
-        d.trace_decay, d.trace_scale = _f(layer.trace_decay), _f(layer.trace_scale)      # nodes.py:129-131
+        d.trace_decay, d.trace_scale = _g("trace_decay"), _g("trace_scale")               # nodes.py:129-131
         d.x = layer.x.data_ptr()
     if layer.sum_input:
         d.summed = layer.summed.data_ptr()
@@ -76,13 +78,13 @@ def fill_layer(d: "_abi.SnnLayer", layer, B: int, keep: List[torch.Tensor]) -> N
     d.s = _u8(layer.s).data_ptr()
     if kind != _abi.SNN_NODE_INPUT:
         d.v = layer.v.data_ptr()
-        d.thresh = _f(layer.thresh)
+        d.thresh = _g("thresh")
         if kind != _abi.SNN_NODE_MCP:                                                     # McCullochPitts: v = x, no other state
             d.refrac_count, d.refrac = layer.refrac_count.data_ptr(), _f(layer.refrac)
         if hasattr(layer, "decay") and kind not in (_abi.SNN_NODE_IF, _abi.SNN_NODE_MCP):
-            d.decay = _f(layer.decay)                                                     # nodes.py:546-548, 1128-1130
+            d.decay = _g("decay")                                                         # nodes.py:546-548, 1128-1130
         if hasattr(layer, "rest"):
-            d.rest = _f(layer.rest)
+            d.rest = _g("rest")
         if hasattr(layer, "reset"):
             d.reset = _f(layer.reset)
         lb = getattr(layer, "lbound", None)
@@ -91,8 +93,40 @@ def fill_layer(d: "_abi.SnnLayer", layer, B: int, keep: List[torch.Tensor]) -> N
         d.i, d.i_decay = layer.i.data_ptr(), _f(layer.i_decay)                            # nodes.py:771, 818-820
     if kind == _abi.SNN_NODE_DC:
         d.theta = layer.theta.data_ptr()
-        d.theta_plus, d.theta_decay = _f(layer.theta_plus), _f(layer.theta_decay)         # nodes.py:1131-1133
+        d.theta_plus, d.theta_decay = _g("theta_plus"), _g("theta_decay")                 # nodes.py:1131-1133
         d.one_spike = int(getattr(layer, "one_spike", False))
+    if rows:   # the per-neuron block (include/snn_b200.h SNN_NODE_PN), [SNN_PN_ROWS, n] fp32 beside v
+        block = torch.zeros(_abi.SNN_PN_ROWS, d.n, dtype=torch.float32, device=layer.v.device)
+        for name, (r, t) in rows.items():
+            block[r].copy_(t.detach().float().expand(tuple(layer.shape)).reshape(-1))
+        keep.append(block)
+        d.kind |= _abi.SNN_NODE_PN
+        d.pn, d.pn_mask = block.data_ptr(), sum(1 << r for r, _ in rows.values())
+
+
+def _neuron_rows(layer, kind: int) -> Dict[str, tuple]:
+    """The parameters of a LIFNodes / AdaptiveLIFNodes / DiehlAndCookNodes population that are tensors of more than one
+    element, by buffer name: {name: (SNN_PN_* row, tensor)}.  refrac / reset / lbound and a non-additive trace_scale
+    reach masked_fill_, which takes a 0-dim value only: the reference's first step raises that RuntimeError."""
+    if kind not in (_abi.SNN_NODE_LIF, _abi.SNN_NODE_DC):
+        return {}
+    many = lambda t: isinstance(t, torch.Tensor) and t.numel() != 1
+    for name in ("refrac", "reset", "lbound") + (() if layer.traces_additive else ("trace_scale",)):
+        t = getattr(layer, name, None)
+        if layer.traces or name != "trace_scale":
+            if many(t):
+                raise RuntimeError(f"masked_fill_ only supports a 0-dimensional value tensor, but got tensor with {t.dim()} "
+                                   f"dimension(s). ('{name}' is a per-neuron tensor)")
+    names = [("thresh", _abi.SNN_PN_THRESH), ("rest", _abi.SNN_PN_REST), ("decay", _abi.SNN_PN_DECAY)]
+    if kind == _abi.SNN_NODE_DC:
+        names += [("theta_plus", _abi.SNN_PN_THETA_PLUS), ("theta_decay", _abi.SNN_PN_THETA_DECAY)]
+    if layer.traces:
+        names += [("trace_decay", _abi.SNN_PN_TRACE_DECAY)] + ([("trace_scale", _abi.SNN_PN_TRACE_SCALE)] if layer.traces_additive else [])
+    rows = {name: (r, getattr(layer, name)) for name, r in names if many(getattr(layer, name))}
+    for name, (_, t) in rows.items():
+        if torch.broadcast_shapes(tuple(t.shape), tuple(layer.shape)) != tuple(layer.shape):
+            raise NotImplementedError(f"per-neuron '{name}' of shape {tuple(t.shape)} grows the layer's state {tuple(layer.shape)}")
+    return rows
 
 
 def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep: Optional[List[torch.Tensor]] = None,

@@ -62,6 +62,32 @@ extern "C" {
                                   x is not in {0, 1} raises SNN_ERR_NONBINARY.  The only connection into such a layer is an
                                   SNN_CONN_MAXPOOL2D, and a connection with such an endpoint has rule SNN_RULE_NONE or
                                   SNN_RULE_NOOP.  Generic tier only */
+/* Per-neuron parameters of an SNN_NODE_LIF or SNN_NODE_DC layer (a parameter given to LIFNodes, AdaptiveLIFNodes or
+ * DiehlAndCookNodes as a tensor, which the reference broadcasts elementwise against [B, *shape]).  The flag is OR-ed into
+ * snn_layer_t.kind; such a layer's pn points to a float32 [k, n] block whose row r holds parameter r of every neuron
+ * (r < k for every bit r of pn_mask) and takes the place of the scalar field wherever the layer reads it:
+ *   SNN_PN_THRESH       thresh       s = v >= thresh[j]  (DC: v >= fl(thresh[j] + theta[j]))
+ *   SNN_PN_REST         rest         v = fl(decay[j] * fl(v - rest[j])) + rest[j]
+ *   SNN_PN_DECAY        decay        exp(-dt / tc_decay[j]) evaluated in fp32 like nodes.py:546-548
+ *   SNN_PN_THETA_PLUS   theta_plus   theta[j] += fl(theta_plus[j] * count), count = the step's spikes summed over the batch (DC)
+ *   SNN_PN_THETA_DECAY  theta_decay  theta[j] *= theta_decay[j] (DC)
+ *   SNN_PN_TRACE_DECAY  trace_decay  x *= trace_decay[j]  (traces only)
+ *   SNN_PN_TRACE_SCALE  trace_scale  x += fl(trace_scale[j] * s)  (traces_additive only: the reference's masked_fill_
+ *                                    takes no tensor value)
+ * A bit the kind does not have (THETA_* on SNN_NODE_LIF, TRACE_* without traces, TRACE_SCALE without traces_additive), a
+ * NULL pn with a non-zero mask or a flag on another kind is SNN_ERR_BAD_ARG.  Generic tier only: tier 0 selects tier 1,
+ * a forced tier 2 or 3 (and so a delta window) is SNN_ERR_UNSUPPORTED; not in a plan that also holds an SNN_CONN_SPARSE
+ * connection, MCC features or a kind of the pooling instantiation.  A library older than the flag refuses such a plan
+ * (it rejects every kind above SNN_NODE_PASSTHROUGH with SNN_ERR_UNSUPPORTED). */
+#define SNN_NODE_PN 0x100
+#define SNN_PN_THRESH 0
+#define SNN_PN_REST 1
+#define SNN_PN_DECAY 2
+#define SNN_PN_THETA_PLUS 3
+#define SNN_PN_THETA_DECAY 4
+#define SNN_PN_TRACE_DECAY 5
+#define SNN_PN_TRACE_SCALE 6
+#define SNN_PN_ROWS 7
 
 /* ---- connection kinds (reference: bindsnet/network/topology.py) ---- */
 #define SNN_CONN_DENSE 0 /* Connection: s.float() @ w + b                topology.py:332-346 */
@@ -209,9 +235,18 @@ typedef struct snn_layer {
     int32_t *rec_count; /* [B,n] += number of spikes of each neuron over the window (what the
                            reference's callers compute as spikes.sum(time), e.g.
                            examples/mnist/batch_eth_mnist.py:280-284); NULL = not counted */
-    /* SNN_NODE_CURRENT_LIF */
-    float *i;           /* [B,n] synaptic input current, updated in place (nodes.py:771,778) */
-    float i_decay;      /* exp(-dt/tc_i_decay) (nodes.py:818-820) */
+    /* SNN_NODE_CURRENT_LIF: the synaptic current.  An SNN_NODE_LIF / SNN_NODE_DC layer never reads these fields, so the
+       same storage carries its per-neuron parameter block when its kind has the SNN_NODE_PN flag (see there). */
+    union {
+        struct {
+            float *i;           /* [B,n] synaptic input current, updated in place (nodes.py:771,778) */
+            float i_decay;      /* exp(-dt/tc_i_decay) (nodes.py:818-820) */
+        };
+        struct {
+            const float *pn;    /* SNN_NODE_PN: float32 [k, n], row r = the SNN_PN_* parameter r of every neuron */
+            uint32_t pn_mask;   /* SNN_NODE_PN: bit r set = row r replaces the scalar field of parameter r */
+        };
+    };
 } snn_layer_t;
 
 /* One dense synapse matrix.  Reference: Connection (topology.py:265-399) or

@@ -98,8 +98,9 @@ struct DevNet {
     DevSparse sp[SNN_MAX_CONNS];
     int32_t any_feat;             // some MCC connection carries Probability / Mask / Intensity features
     int32_t any_pool;             // some connection is a MaxPool2dConnection (SNN_CONN_MAXPOOL2D), a LocalConnection2D
-                                  // (SNN_CONN_LOCAL2D) or a Conv3dConnection (SNN_CONN_CONV3D), or some layer is an
-                                  // SNN_NODE_SUBIF / SNN_NODE_PASSTHROUGH one: the plan runs the POOL instantiation
+                                  // (SNN_CONN_LOCAL2D), a Conv3dConnection (SNN_CONN_CONV3D) or a Conv1dConnection
+                                  // (SNN_CONN_CONV1D), or some layer is an SNN_NODE_SUBIF / SNN_NODE_PASSTHROUGH one: the
+                                  // plan runs the POOL instantiation
     float *pool_r1[SNN_MAX_CONNS];   // MaxPool2dConnection: the workspace slot of its rates (pool_rate_slot)
 };
 
@@ -152,6 +153,20 @@ static inline int snn_conv3d_geometry_ok(const snn_conn_t &C, int n_src, int n_t
         return SNN_ERR_BAD_ARG;
     if ((long long)C.cin * C.din * C.hin * C.win != n_src || (long long)C.cout * C.dout * C.hout * C.wout != n_tgt) return SNN_ERR_BAD_ARG;
     return SNN_OK;
+}
+// A Conv1dConnection's geometry (snn_b200.h): the layer sizes, the output size of a kernel that fits the padded input,
+// the height axis set to 1, no dilation, w and b present.
+static inline int snn_conv1d_geometry_ok(const snn_conn_t &C, int n_src, int n_tgt) {
+    if (!C.w || !C.b) return SNN_ERR_BAD_ARG;
+    if (C.cin < 1 || C.cout < 1 || C.kw < 1 || C.sw < 1 || C.pw < 0 || C.win < 1 || C.wout < 1) return SNN_ERR_BAD_ARG;
+    if (C.hin != 1 || C.hout != 1 || C.kh != 1 || C.sh != 1 || C.ph != 0 || C.dh != 1 || C.dw != 1) return SNN_ERR_BAD_ARG;
+    if (C.wout != snn_conv3d_out(C.win, C.kw, C.sw, C.pw)) return SNN_ERR_BAD_ARG;
+    if ((long long)C.cin * C.win != n_src || (long long)C.cout * C.wout != n_tgt) return SNN_ERR_BAD_ARG;
+    return SNN_OK;
+}
+static inline bool snn_conv1d_rule_ok(const snn_conn_t &C) {
+    return C.rule == SNN_RULE_NONE || C.rule == SNN_RULE_NOOP || C.rule == SNN_RULE_POSTPRE || C.rule == SNN_RULE_WDEP_POSTPRE ||
+           C.rule == SNN_RULE_HEBBIAN;
 }
 // The updates a Conv3dConnection runs (snn_b200.h): none, learning.NoOp's decay, or a zero-rate PostPre /
 // WeightDependentPostPre (decay and clamp).

@@ -166,6 +166,29 @@ __global__ void __launch_bounds__(256) conv3d_compute_kernel(snn_conn_t C, int n
 
 __global__ void __launch_bounds__(SNN_GEN_THREADS) conv3d_update_kernel(snn_conn_t C) { phase3_conv3d(C, blockIdx.x, gridDim.x); }
 
+// Conv1dConnection.compute (topology.py:640-656) on byte spikes: the window gather's gather_conv1d order ((ci, kx)
+// ascending from +0, then the bias).  Thread = one target neuron of one sample.
+__global__ void __launch_bounds__(256) conv1d_compute_kernel(snn_conn_t C, int ns, int nt, int B, const uint8_t *__restrict__ s,
+                                                             float *__restrict__ out) {
+    const size_t total = (size_t)B * nt;
+    for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+        const int b = (int)(e / nt), j = (int)(e - (size_t)b * nt), co = j / C.wout, ox = j - co * C.wout;
+        const uint8_t *sb = s + (size_t)b * ns;
+        const float *wf = C.w + (size_t)co * C.cin * C.kw;
+        float p = 0.0f;
+        for (int ci = 0; ci < C.cin; ++ci)
+            for (int kx = 0; kx < C.kw; ++kx) {
+                const int ix = ox * C.sw - C.pw + kx;
+                if (ix >= 0 && ix < C.win && sb[ci * C.win + ix]) p = p + wf[ci * C.kw + kx];
+            }
+        out[e] = p + C.b[co];
+    }
+}
+
+__global__ void __launch_bounds__(SNN_GEN_THREADS) conv1d_update_kernel(const __grid_constant__ DevNet N, int ci) {
+    phase3_conv1d(N, ci, blockIdx.x, gridDim.x, 0);
+}
+
 // LocalConnection2D.compute (topology.py:1717-1740) on byte spikes: the window gather's gather_local2d order (k ascending
 // within a channel from +0, then the channels).  Thread = one target neuron of one sample.
 __global__ void __launch_bounds__(256) local2d_compute_kernel(snn_conn_t C, int ns, int nt, int B, const uint8_t *__restrict__ s,
@@ -305,6 +328,14 @@ int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, 
         SNN_LAUNCH(conv3d_compute_kernel, blocks, 256, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
         return cuda_rc(cudaGetLastError());
     }
+    if (conn->kind == SNN_CONN_CONV1D) {
+        const int rc = snn_conv1d_geometry_ok(*conn, n_src, n_tgt);
+        if (rc != SNN_OK) return rc;
+        const size_t total = (size_t)B * n_tgt;
+        const int blocks = (int)((total + 255) / 256 < 4736 ? (total + 255) / 256 : 4736);
+        SNN_LAUNCH(conv1d_compute_kernel, blocks, 256, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
+        return cuda_rc(cudaGetLastError());
+    }
     if (conn->kind == SNN_CONN_CONV2D) {
         if (!conn->b || conn->cin * conn->hin * conn->win != n_src || conn->cout * conn->hout * conn->wout != n_tgt) return SNN_ERR_BAD_ARG;
         const size_t total = (size_t)B * n_tgt;
@@ -354,12 +385,17 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
     if (pass && C.rule != SNN_RULE_NONE && C.rule != SNN_RULE_NOOP) return SNN_ERR_UNSUPPORTED;   // (snn_b200.h)
     // the single-operator update is the dense [n_src, n_tgt] rule application or a LocalConnection2D's; convolutional
     // weights and the reward-modulated rules (whose state lives in the window plan) are only updated inside run_window
-    const bool local = C.kind == SNN_CONN_LOCAL2D;
-    if (C.kind != SNN_CONN_DENSE && C.kind != SNN_CONN_MCC && !local) return SNN_ERR_UNSUPPORTED;
+    const bool local = C.kind == SNN_CONN_LOCAL2D, conv1d = C.kind == SNN_CONN_CONV1D;
+    if (C.kind != SNN_CONN_DENSE && C.kind != SNN_CONN_MCC && !local && !conv1d) return SNN_ERR_UNSUPPORTED;
     if (local) {
         const int rc = snn_local2d_geometry_ok(C, net->layers[C.src].n, net->layers[C.tgt].n);
         if (rc != SNN_OK) return rc;
         if (C.rule == SNN_RULE_MCC_POSTPRE) return SNN_ERR_UNSUPPORTED;
+    }
+    if (conv1d) {
+        const int rc = snn_conv1d_geometry_ok(C, net->layers[C.src].n, net->layers[C.tgt].n);
+        if (rc != SNN_OK) return rc;
+        if (!snn_conv1d_rule_ok(C) || C.mask) return SNN_ERR_UNSUPPORTED;
     }
     if (SNN_RULE_IS_MSTDP(C.rule)) return SNN_ERR_UNSUPPORTED;
     const bool syn = snn_has_syn(C);
@@ -395,6 +431,12 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
         SNN_LAUNCH(local2d_update_kernel, blocks, SNN_GEN_THREADS, 0, stream, N, ci);
         return cuda_rc(cudaGetLastError());
     }
+    if (conv1d) {   // one warp per group of elements, like the window's learning phase
+        const size_t NW = (size_t)C.cout * C.cin * C.kw;
+        const int blocks = (int)((NW + SNN_GEN_WARPS - 1) / SNN_GEN_WARPS < 1184 ? (NW + SNN_GEN_WARPS - 1) / SNN_GEN_WARPS : 1184);
+        SNN_LAUNCH(conv1d_update_kernel, blocks, SNN_GEN_THREADS, 0, stream, N, ci);
+        return cuda_rc(cudaGetLastError());
+    }
     const size_t smem = gen_smem_bytes(B);
     if (syn) {
         cudaFuncSetAttribute(conn_update_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -425,6 +467,11 @@ int snn_b200_conn_normalize(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt
         const int F = conn->cout * conn->cin;
         SNN_LAUNCH(conv_normalize_kernel, (F + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn,
                    conn->kd * conn->kh * conn->kw);
+        return cuda_rc(cudaGetLastError());
+    }
+    if (conn->kind == SNN_CONN_CONV1D) {   // rows of w viewed as [cout * cin, kw]
+        const int F = conn->cout * conn->cin;
+        SNN_LAUNCH(conv_normalize_kernel, (F + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, conn->kw);
         return cuda_rc(cudaGetLastError());
     }
     SNN_LAUNCH(conn_normalize_kernel, (n_tgt + SNN_TILE - 1) / SNN_TILE, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, n_src, n_tgt);

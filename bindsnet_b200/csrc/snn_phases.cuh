@@ -410,6 +410,34 @@ __device__ __forceinline__ float gather_conv3d(const snn_conn_t &C, const uint32
     return p + C.b[co];
 }
 
+// Conv1dConnection.compute (topology.py:640-656) for one target neuron j = (co, ox) of one sample: the sum of the taps
+// whose (zero-padded) input position spiked, in ascending (ci, kx) order from +0, then the bias.  Each channel's valid
+// tap run [kx_lo, kx_hi) looks at consecutive source bits: it is cut out of the bit row 32 bits at a time with a funnel
+// shift (any kernel length) and only its set bits are visited.  STAGED_BITS / STAGED_TAPS as for gather_conv3d.
+template <bool STAGED_BITS, bool STAGED_TAPS>
+__device__ __forceinline__ float gather_conv1d(const snn_conn_t &C, const uint32_t *sb, const float *taps, int co_base, int j, bool valid) {
+    if (!valid) return 0.0f;
+    const int co = j / C.wout, ox = j - co * C.wout, ix0 = ox * C.sw - C.pw;
+    const int kx_lo = max(0, -ix0), kx_hi = min(C.kw, C.win - ix0);
+    const float *tp = STAGED_TAPS ? taps + (size_t)(co - co_base) * C.cin * C.kw : C.w + (size_t)co * C.cin * C.kw;
+    float p = 0.0f;
+    for (int ci = 0; ci < C.cin; ++ci) {
+        const int row = ci * C.win + ix0, k0 = ci * C.kw;   // source bit of tap kx = 0, its tap index
+        for (int kx = kx_lo; kx < kx_hi; kx += 32) {
+            const int cnt = min(32, kx_hi - kx), bit0 = row + kx, w0 = bit0 >> 5, sft = bit0 & 31;
+            const uint32_t lo = STAGED_BITS ? sb[w0] : __ldcg(sb + w0);
+            const uint32_t hi = sft + cnt > 32 ? (STAGED_BITS ? sb[w0 + 1] : __ldcg(sb + w0 + 1)) : 0u;
+            uint32_t bits = __funnelshift_r(lo, hi, sft) & (cnt >= 32 ? 0xffffffffu : ((1u << cnt) - 1u));
+            while (bits) {
+                const int k = k0 + kx + __ffs(bits) - 1;
+                bits &= bits - 1;
+                p = p + (STAGED_TAPS ? tp[k] : __ldcg(tp + k));
+            }
+        }
+    }
+    return p + C.b[co];
+}
+
 // LocalConnection2D.compute (topology.py:1717-1740) for target neuron j = (f, oy, ox) of one sample (n target neurons):
 // per input channel the sum of its own weights w[ci, j, k] whose window position k spiked (k ascending, from +0), then
 // the channel sums in ascending ci (the reference's sum(-1).sum(1)).  The kw window bits of a kernel row are cut out of
@@ -592,14 +620,16 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
     int cnt = 0;  // candidates of this column over this warp's samples
 
     // a convolutional input: stage the chunk's source bit rows and the taps of this tile's output channels (POOL: a
-    // Conv3dConnection input likewise, with the depth axis in its channel size and taps; a LocalConnection2D input gets
-    // its bit rows staged the same way, its weights are per target, not taps)
+    // Conv3dConnection input likewise, with the depth axis in its channel size and taps; a Conv1dConnection input too,
+    // its height axis 1; a LocalConnection2D input gets its bit rows staged the same way, its weights are per target,
+    // not taps)
     int conv_c = -1, conv_slot = 0, co_base = 0;
     bool st_bits = false, st_taps = false;
     ConvGeo geo = {};
     for (int c = 0; c < N.n_conns && conv_c < 0; ++c)
         if (N.conns[c].tgt == li &&
-            (N.conns[c].kind == SNN_CONN_CONV2D || (POOL && (N.conns[c].kind == SNN_CONN_LOCAL2D || N.conns[c].kind == SNN_CONN_CONV3D))))
+            (N.conns[c].kind == SNN_CONN_CONV2D ||
+             (POOL && (N.conns[c].kind == SNN_CONN_LOCAL2D || N.conns[c].kind == SNN_CONN_CONV3D || N.conns[c].kind == SNN_CONN_CONV1D))))
             conv_c = c;
     if (conv_c >= 0) {
         const snn_conn_t &C = N.conns[conv_c];
@@ -650,7 +680,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
             fwn[q] = 0u; afn[q] = 1u;
             if (q < ncl && b < b1 && N.conns[cl[q]].kind != SNN_CONN_CONV2D && !(SPARSE && N.conns[cl[q]].kind == SNN_CONN_SPARSE) &&
                 !(POOL && (N.conns[cl[q]].kind == SNN_CONN_MAXPOOL2D || N.conns[cl[q]].kind == SNN_CONN_LOCAL2D ||
-                           N.conns[cl[q]].kind == SNN_CONN_CONV3D))) {
+                           N.conns[cl[q]].kind == SNN_CONN_CONV3D || N.conns[cl[q]].kind == SNN_CONN_CONV1D))) {
                 const snn_conn_t &C = N.conns[cl[q]];
                 const DevLayer &S = N.layers[C.src];
                 const int slot = (N.one_step && C.src < li) ? wr : rd;
@@ -716,6 +746,16 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
                     p = gather_conv3d<false, true>(C, gsb, M.xs, co_base, j, valid);
                 } else {
                     p = gather_conv3d<false, false>(C, gsb, nullptr, 0, j, valid);
+                }
+            } else if (POOL && C.kind == SNN_CONN_CONV1D) {
+                const uint32_t *gsb = S.bits + ((size_t)slot * B + b) * S.nw;
+                if (c == conv_c && st_bits) {
+                    const uint32_t *ssb = M.cbits + (size_t)(b - b0) * S.nw;
+                    p = st_taps ? gather_conv1d<true, true>(C, ssb, M.xs, co_base, j, valid) : gather_conv1d<true, false>(C, ssb, nullptr, 0, j, valid);
+                } else if (c == conv_c && st_taps) {
+                    p = gather_conv1d<false, true>(C, gsb, M.xs, co_base, j, valid);
+                } else {
+                    p = gather_conv1d<false, false>(C, gsb, nullptr, 0, j, valid);
                 }
             } else if (POOL && C.kind == SNN_CONN_LOCAL2D) {
                 p = c == conv_c && st_bits ? gather_local2d<true>(C, M.cbits + (size_t)(b - b0) * S.nw, n, j, valid)
@@ -1346,6 +1386,81 @@ __device__ void phase3_conv3d(const snn_conn_t &C, int cta, int ncta) {
         if (C.weight_decay != 0.0f) x = x * C.weight_decay;
         if (clamp) x = clampf(x, C.wmin, C.wmax);
         C.w[e] = x;
+    }
+}
+
+// PostPre / WeightDependentPostPre / Hebbian on a Conv1dConnection (learning.py:422-455, 873-918, 1316-1346), and the
+// decay of learning.NoOp.  Element e = co * cin * kw + m takes (snn_b200.h)
+//   U = reduce_b sum_l' x_tgt[b, co, l'] * s_src[b, src(l', m)],  V = reduce_b sum_l' s_tgt[b, co, l'] * x_src[b, src(l', m)]
+// where src is the source neuron the reference's reshape of the unfolded source pairs with target position l'.  Along
+// l' that pairing keeps kk' = m % kw and advances the unfolded row l by cin (wrapping into the next channel c), so it is
+// stepped, not divided out.  One warp per group of 32 / g elements, g lanes per element over the samples (g = B rounded
+// up to a power of two, at most 32): each lane builds its sample's partial sums over l' ascending, visiting the target
+// bits a word at a time and skipping the terms of silent spikes; the partials then join in ascending b through
+// shuffles, g samples at a time.  Traces are read from the layers' own arrays, framed by the grid barriers around the
+// learning phase.
+__device__ void phase3_conv1d(const DevNet &N, int ci_, int cta, int ncta, int t) {
+    const snn_conn_t &C = N.conns[ci_];
+    const DevLayer &S = N.layers[C.src], &G = N.layers[C.tgt];
+    const int B = N.B, ns = S.L.n, nt = G.L.n, Mw = C.cin * C.kw, L = C.wout, NW = C.cout * Mw;
+    if (!SNN_RULE_IS_STDP(C.rule)) {   // learning.NoOp: w *= weight_decay (learning.py:93-94), no clamp
+        if (C.weight_decay != 0.0f)
+            for (int e = cta * SNN_GEN_THREADS + threadIdx.x; e < NW; e += ncta * SNN_GEN_THREADS) C.w[e] = __ldcg(C.w + e) * C.weight_decay;
+        return;
+    }
+    const bool hebb = C.rule == SNN_RULE_HEBBIAN;
+    const bool pre_on = C.nu0 != 0.0f || hebb, post_on = C.nu1 != 0.0f || hebb;
+    const int wr = t & 1, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int g = 1;
+    while (g < B && g < 32) g <<= 1;
+    const int epw = 32 / g, base = lane & ~(g - 1), sub = lane - base, LK = L * C.kw;
+    for (int e0 = (cta * SNN_GEN_WARPS + warp) * epw; e0 < NW; e0 += ncta * SNN_GEN_WARPS * epw) {
+        const int e = e0 + lane / g;
+        const bool ok = e < NW;
+        const int co = ok ? e / Mw : 0, m = ok ? e - co * Mw : 0;
+        const int c0 = m / LK, r0 = m - c0 * LK, l0 = r0 / C.kw, off = r0 - l0 * C.kw - C.pw;   // the pairing at l' = 0
+        float U = 0.0f, V = 0.0f;
+        for (int bq = 0; bq < B; bq += g) {
+            const int b = bq + sub;
+            float u1 = 0.0f, v1 = 0.0f;
+            if (ok && b < B) {
+                const uint32_t *sb = S.bits + ((size_t)wr * B + b) * S.nw, *gb = G.bits + ((size_t)wr * B + b) * G.nw;
+                const float *xt = G.L.x + (size_t)b * nt + (size_t)co * L, *xs = S.L.x + (size_t)b * ns;
+                int c = c0, l = l0, cw = -1;
+                uint32_t cword = 0u;   // the source bit word last read (word cw)
+                for (int lq = 0; lq < L; lq += 32) {
+                    const int cnt = min(32, L - lq), bit0 = co * L + lq, w0 = bit0 >> 5, sft = bit0 & 31;
+                    uint32_t tw = 0u;   // target spikes of l' in [lq, lq + cnt)
+                    if (post_on) {
+                        const uint32_t lo = __ldcg(gb + w0), hi = sft + cnt > 32 ? __ldcg(gb + w0 + 1) : 0u;
+                        tw = __funnelshift_r(lo, hi, sft) & (cnt >= 32 ? 0xffffffffu : ((1u << cnt) - 1u));
+                    }
+                    for (int q = 0; q < cnt; ++q) {
+                        const int pos = l * C.sw + off;
+                        if (pos >= 0 && pos < C.win) {
+                            const int src = c * C.win + pos;
+                            if (pre_on) {
+                                if ((src >> 5) != cw) { cw = src >> 5; cword = __ldcg(sb + cw); }
+                                if ((cword >> (src & 31)) & 1u) u1 = u1 + __ldcg(xt + lq + q);
+                            }
+                            if ((tw >> q) & 1u) v1 = v1 + __ldcg(xs + src);
+                        }
+                        l += C.cin;
+                        while (l >= L) { l -= L; ++c; }
+                    }
+                }
+            }
+            const int nb = min(g, B - bq);
+            for (int q = 0; q < nb; ++q) {
+                const float uq = __shfl_sync(0xffffffffu, u1, base + q), vq = __shfl_sync(0xffffffffu, v1, base + q);
+                U = U + uq;
+                V = V + vq;
+            }
+        }
+        if (ok && sub == 0) {
+            if (C.reduction == SNN_REDUCE_MEAN) { U = U / (float)B; V = V / (float)B; }
+            C.w[e] = stdp_rule_apply(C, __ldcg(C.w + e), U, V, pre_on, post_on);
+        }
     }
 }
 

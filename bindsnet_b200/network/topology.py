@@ -352,6 +352,118 @@ class Conv2dConnection(AbstractConnection):
             self.update_rule._fill_desc(d)
 
 
+class Conv1dConnection(AbstractConnection):
+    """1-D convolutional synapses (reference: topology.py:540-683) between ``[C, L]`` populations.  ``w`` is
+    ``[out_channels, in_channels, kernel_size]``, ``b`` ``[out_channels]`` (zeros by default).  Inside ``Network.run`` the
+    convolution is a spike-gather over each target neuron's receptive field, and ``PostPre``, ``WeightDependentPostPre``,
+    ``Hebbian`` or ``NoOp`` update ``w`` on the generic window kernel; ``normalize`` scales every ``(out, in)`` filter to
+    sum ``norm``.
+
+    As in the reference: a dilation other than 1 raises ``NotImplementedError``; a target whose shape is not
+    ``[out_channels, int((L - k + 2p) / s + 1)]`` raises ``AssertionError``; ``w`` is drawn with ``torch.rand`` and clamped
+    or scaled like ``Conv2dConnection``'s.  The rules' update follows the reference's reshape of the unfolded source,
+    which for ``in_channels > 1`` pairs a weight with another source neuron than ``compute`` does (include/snn_b200.h,
+    SNN_CONN_CONV1D).  Only ``[C, L]`` source and target populations are built: any other shape raises
+    ``NotImplementedError`` before anything else (the reference's ``F.conv1d`` cannot take the batch such a source gives;
+    DESIGN.md section 8).  ``MSTDP`` / ``MSTDPET`` on it raise ``NotImplementedError``."""
+
+    def __init__(
+        self,
+        source: Nodes,
+        target: Nodes,
+        kernel_size: int,
+        stride: int = 1,
+        padding: int = 0,
+        dilation: int = 1,
+        nu: Optional[Union[float, Sequence[float], Sequence[torch.Tensor]]] = None,
+        reduction: Optional[callable] = None,
+        weight_decay: float = 0.0,
+        w_dtype: torch.dtype = torch.float32,
+        **kwargs,
+    ) -> None:
+        for name, layer in (("source", source), ("target", target)):
+            if not isinstance(layer, Nodes) or len(layer.shape) != 2:
+                shape = list(layer.shape) if isinstance(layer, Nodes) else type(layer).__name__
+                raise NotImplementedError(f"Conv1dConnection is built between [C, L] populations only; the {name} is {shape}")
+        if w_dtype != torch.float32:
+            raise NotImplementedError("bindsnet_b200 computes in float32 only (SURVEY.md §8b)")
+        super().__init__(source, target, nu, reduction, weight_decay, **kwargs)
+        if dilation != 1:                                                                   # topology.py:592-595
+            raise NotImplementedError("Dilation is not currently supported for 1-D spiking convolution.")
+        self.kernel_size, self.stride, self.padding, self.dilation = kernel_size, stride, padding, dilation
+        self.in_channels, input_size = source.shape[0], source.shape[1]
+        self.out_channels, output_size = target.shape[0], target.shape[1]
+        conv_size = (input_size - self.kernel_size + 2 * self.padding) / self.stride + 1       # topology.py:605-613
+        assert target.shape[0] == self.out_channels and target.shape[1] == int(conv_size), (
+            "Target dimensionality must be (out_channels, ?,(input_size - filter_size + 2 * padding) / stride + 1,"
+        )
+        w = kwargs.get("w", None)
+        shape = (self.out_channels, self.in_channels, self.kernel_size)
+        if w is None:
+            # topology.py:615-629
+            if (self.wmin == -np.inf).any() or (self.wmax == np.inf).any():
+                w = torch.clamp(torch.rand(*shape), self.wmin, self.wmax)
+            else:
+                w = (self.wmax - self.wmin) * torch.rand(*shape)
+                w = w + self.wmin
+        else:
+            # topology.py:630-633
+            w = torch.as_tensor(w)
+            if (self.wmin == -np.inf).any() or (self.wmax == np.inf).any():
+                w = torch.clamp(w, self.wmin, self.wmax)
+            w = self.cast_dtype_if_needed(w, w_dtype)
+        self.w = Parameter(w.detach().clone().float().contiguous(), requires_grad=False)
+        self.b = Parameter(torch.as_tensor(kwargs.get("b", torch.zeros(self.out_channels)), dtype=torch.float32).clone(),
+                           requires_grad=False)
+
+    def compute(self, s: torch.Tensor) -> torch.Tensor:
+        """``F.conv1d(s.float(), w, b, stride, padding)`` for {0,1} spikes (topology.py:640-656), as the spike-gather the
+        window kernel uses (``snn_b200_conn_compute``)."""
+        from . import _plan
+
+        return _plan.compute_single_connection(self, s)
+
+    def normalize(self) -> None:
+        """Every (out, in) filter scaled to sum ``norm`` (topology.py:665-676; a filter that sums to zero becomes
+        inf / NaN, as in the reference); also runs at the end of every ``Network.run`` window."""
+        if self.norm is not None:
+            from . import _plan
+
+            _plan.normalize_single_connection(self)
+
+    def _check(self) -> None:
+        """The errors of the reference's first ``compute`` (F.conv1d), raised before anything runs."""
+        if int(self.target.shape[1]) == 0 or int(self.target.shape[0]) == 0:
+            raise RuntimeError(f"Conv1dConnection: calculated output size {list(self.target.shape)} is too small (kernel "
+                               f"{self.kernel_size}, padded input {int(self.source.shape[1]) + 2 * self.padding})")
+        shape = (int(self.out_channels), int(self.in_channels), int(self.kernel_size))
+        if tuple(self.w.shape) != shape:
+            raise RuntimeError(f"Conv1dConnection.w has shape {tuple(self.w.shape)}, expected {shape}")
+        if tuple(self.b.shape) != (shape[0],):
+            raise RuntimeError(f"Given weight of size {list(self.w.shape)}, expected bias to be 1-dimensional with {shape[0]} "
+                               f"elements, but got bias of size {list(self.b.shape)} instead")
+
+    def _fill_desc(self, d: "_abi.SnnConn", dt: float, rule: bool = True) -> None:
+        self._check()
+        d.kind = _abi.SNN_CONN_CONV1D
+        if self.wmin.numel() != 1 or self.wmax.numel() != 1:
+            raise NotImplementedError("per-synapse wmin/wmax tensors are not supported by the CUDA core yet")
+        d.wmin = _scalar(self.wmin, "wmin")
+        d.wmax = _scalar(self.wmax, "wmax")
+        d.has_norm = int(self.norm is not None)
+        d.norm_abs = 0
+        d.norm = float(self.norm) if self.norm is not None else 0.0
+        d.dt_scale = 1.0
+        d.cin, d.win = (int(v) for v in self.source.shape)
+        d.cout, d.wout = (int(v) for v in self.target.shape)
+        d.kw, d.sw, d.pw = int(self.kernel_size), int(self.stride), int(self.padding)
+        d.hin = d.hout = d.kh = d.sh = 1
+        d.ph = 0
+        d.dh = d.dw = 1
+        if rule:
+            self.update_rule._fill_desc(d)
+
+
 def _triple(x):
     return tuple(x) if isinstance(x, (tuple, list)) else (x, x, x)
 
@@ -976,7 +1088,6 @@ def _unsupported(name: str, where: str):
     return _Unsupported
 
 
-Conv1dConnection = _unsupported("Conv1dConnection", "topology.py:540-683")
 MaxPool1dConnection = _unsupported("MaxPool1dConnection", "topology.py:1028-1121")
 MaxPoo3dConnection = _unsupported("MaxPoo3dConnection", "topology.py:1214-1301")
 LocalConnection1D = _unsupported("LocalConnection1D", "topology.py:1487-1620")

@@ -10,7 +10,8 @@ a library that implements it — ``libsnn_b200.so`` on CUDA tensors, or the orac
 Covered: what ``bindsnet.models`` builds for the hot path — ``Input`` / ``LIFNodes`` / ``DiehlAndCookNodes`` layers,
 ``MulticompartmentConnection`` with one ``Weight`` feature (``MCC_learning.NoOp`` / ``PostPre``) and the classic
 ``Connection`` and ``LocalConnection2D`` with ``learning.NoOp`` / ``PostPre`` / ``WeightDependentPostPre`` / ``Hebbian``,
-``Conv3dConnection`` with the updates the reference can run on it.  Every attribute is read where the
+``Conv3dConnection`` with the updates the reference can run on it, ``Conv1dConnection`` with ``learning.NoOp`` /
+``PostPre`` / ``WeightDependentPostPre`` / ``Hebbian``.  Every attribute is read where the
 reference keeps it (file:line in the comments); state tensors are handed over by pointer and updated in place.
 """
 from __future__ import annotations
@@ -205,6 +206,35 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
             d.weight_decay = _f(rule.weight_decay)                                        # learning.py:85
             d.wmin, d.wmax = _f(conn.wmin), _f(conn.wmax)
             d.has_clamp = int((math.isfinite(d.wmin) or math.isfinite(d.wmax)) and name != "NoOp")   # learning.py:97-104
+        for t in (conn.w, conn.b):
+            if t.dtype != torch.float32 or not t.is_contiguous():
+                raise TypeError("weights and bias must be contiguous float32")
+        d.w, d.b = conn.w.data_ptr(), conn.b.data_ptr()
+        return
+    if type(conn).__name__ == "Conv1dConnection":
+        # topology.py:540-683: w [out, in, k], b [out]; the geometry of F.conv1d (dilation 1: the constructor refuses any
+        # other) with the height axis set to 1
+        if len(conn.source.shape) != 2 or len(conn.target.shape) != 2:
+            raise NotImplementedError("Conv1dConnection between populations other than [C, L]")
+        d.kind = _abi.SNN_CONN_CONV1D
+        d.cin, d.win = (int(v) for v in conn.source.shape)
+        d.cout, d.wout = (int(v) for v in conn.target.shape)
+        d.kw, d.sw, d.pw = int(conn.kernel_size), int(conn.stride), int(conn.padding)
+        d.hin = d.hout = d.kh = d.sh = 1
+        d.dh = d.dw = 1
+        d.has_norm = int(conn.norm is not None)                                           # topology.py:665-676
+        d.norm, d.norm_abs = (_f(conn.norm) if conn.norm is not None else 0.0), 0
+        rule = conn.update_rule
+        name = type(rule).__name__
+        d.rule = {"NoOp": _abi.SNN_RULE_NOOP, "PostPre": _abi.SNN_RULE_POSTPRE, "Hebbian": _abi.SNN_RULE_HEBBIAN,
+                  "WeightDependentPostPre": _abi.SNN_RULE_WDEP_POSTPRE}.get(name, -1)
+        if d.rule < 0:
+            raise NotImplementedError(f"learning rule {name} on a Conv1dConnection")
+        d.nu0, d.nu1 = _f(rule.nu[0]), _f(rule.nu[1])
+        d.reduction = _reduction_code(rule.reduction)
+        d.weight_decay = _f(rule.weight_decay)                                            # learning.py:85
+        d.wmin, d.wmax = _f(conn.wmin), _f(conn.wmax)
+        d.has_clamp = int((math.isfinite(d.wmin) or math.isfinite(d.wmax)) and name != "NoOp")   # learning.py:97-104
         for t in (conn.w, conn.b):
             if t.dtype != torch.float32 or not t.is_contiguous():
                 raise TypeError("weights and bias must be contiguous float32")

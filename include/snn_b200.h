@@ -139,8 +139,24 @@ extern "C" {
                               rule is SNN_ERR_UNSUPPORTED.  normalize: each row of w viewed as [cout * cin, kd*kh*kw]
                               scaled by norm / (its sum, ascending), no guard against a zero sum.  No mask.  Generic
                               tier only, not with SNN_CONN_SPARSE or MCC features */
-
-/* ---- learning rules ---- */
+#define SNN_CONN_CONV1D 7  /* Conv1dConnection: F.conv1d(s.float(), w, b, stride, padding), topology.py:540-683.
+                              Source [cin,win], target [cout,wout]; w is [cout,cin,kw], b is [cout].  The conv fields
+                              with the height axis set to 1 (hin = hout = kh = sh = 1, ph = 0, dh = dw = 1);
+                              wout = (win - kw + 2pw) / sw + 1 >= 1.  Target (co, ox) receives the sum of the taps whose
+                              zero-padded input position spiked, in ascending (ci, kx) order from +0, then + b[co].
+                              Rules SNN_RULE_NONE / NOOP / POSTPRE / WDEP_POSTPRE / HEBBIAN.  The rules' element (co, m),
+                              m = ci * kw + kk < cin * kw, is flat weight co * cin * kw + m; it pairs target position l'
+                              (L = wout) with the source neuron the reference's reshape of the unfolded source
+                              [cin, L, kw] to [L, cin * kw] puts there: f = l' * cin * kw + m, c = f / (L * kw),
+                              l = (f % (L * kw)) / kw, kk' = f % kw, source c * win + l * sw - pw + kk' (a padding
+                              position: no term).  For cin = 1 this is the convolution's own pairing.
+                                U = reduce_b sum_l' x_tgt[b, co, l'] * s_src[b, src],
+                                V = reduce_b sum_l' s_tgt[b, co, l'] * x_src[b, src]
+                              each sample's sum in ascending l', the samples' sums in ascending b, the terms of a silent
+                              spike skipped; then PostPre / WeightDependentPostPre / Hebbian as on SNN_CONN_CONV2D,
+                              decay and clamp.  normalize: each row of w viewed as [cout * cin, kw] scaled by
+                              norm / (its sum, ascending), no guard against a zero sum.  No mask.  Generic tier only,
+                              not with SNN_CONN_SPARSE or MCC features */
 #define SNN_RULE_NONE 0        /* MCC_learning.NoOp: update() does nothing    MCC_learning.py:120-146 */
 #define SNN_RULE_NOOP 1        /* learning.NoOp: weight decay only, no clamp  learning.py:107-146     */
 #define SNN_RULE_POSTPRE 2     /* learning.PostPre._connection_update         learning.py:390-420     */

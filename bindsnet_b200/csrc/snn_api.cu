@@ -74,12 +74,12 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
     for (int c = 0; c < net->n_conns; ++c) {
         const snn_conn_t &C = net->conns[c];
         const bool sparse = C.kind == SNN_CONN_SPARSE, pool = C.kind == SNN_CONN_MAXPOOL2D, local = C.kind == SNN_CONN_LOCAL2D;
-        const bool conv3d = C.kind == SNN_CONN_CONV3D, conv1d = C.kind == SNN_CONN_CONV1D;
+        const bool conv3d = C.kind == SNN_CONN_CONV3D, conv1d = C.kind == SNN_CONN_CONV1D, local3d = C.kind == SNN_CONN_LOCAL3D;
         if (C.src < 0 || C.src >= net->n_layers || C.tgt < 0 || C.tgt >= net->n_layers) return SNN_ERR_BAD_ARG;
         if (pool ? (C.w || C.b) : (!C.w && !(sparse && C.nnz == 0))) return SNN_ERR_BAD_ARG;
         if (net->layers[C.tgt].kind == SNN_NODE_INPUT) return SNN_ERR_UNSUPPORTED;
         if (C.rule < SNN_RULE_NONE || C.rule > SNN_RULE_MSTDPET) return SNN_ERR_UNSUPPORTED;
-        if (C.kind < SNN_CONN_DENSE || C.kind > SNN_CONN_CONV1D) return SNN_ERR_UNSUPPORTED;
+        if (C.kind < SNN_CONN_DENSE || C.kind > SNN_CONN_LOCAL3D) return SNN_ERR_UNSUPPORTED;
         if (conv1d) {   // NoOp and the three unsupervised rules, no mask (snn_b200.h)
             const int rc = snn_conv1d_geometry_ok(C, net->layers[C.src].n, net->layers[C.tgt].n);
             if (rc != SNN_OK) return rc;
@@ -96,6 +96,11 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
             if (C.rule != SNN_RULE_NONE && C.rule != SNN_RULE_NOOP && C.rule != SNN_RULE_POSTPRE && C.rule != SNN_RULE_WDEP_POSTPRE &&
                 C.rule != SNN_RULE_HEBBIAN)
                 return SNN_ERR_UNSUPPORTED;
+        }
+        if (local3d) {   // as a LocalConnection2D, on three axes (snn_b200.h)
+            const int rc = snn_local3d_geometry_ok(C, net->layers[C.src].n, net->layers[C.tgt].n);
+            if (rc != SNN_OK) return rc;
+            if (!snn_local_rule_ok(C) || C.mask) return SNN_ERR_UNSUPPORTED;
         }
         if (conv3d) {   // decay / clamp updates only, no mask (snn_b200.h)
             const int rc = snn_conv3d_geometry_ok(C, net->layers[C.src].n, net->layers[C.tgt].n);
@@ -143,11 +148,11 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
 }
 
 // the plan runs the pooling instantiation of the generic kernel: a MaxPool2dConnection, a LocalConnection2D, a
-// Conv3dConnection, a Conv1dConnection, or a layer of ann_to_snn's kinds
+// Conv3dConnection, a Conv1dConnection, a LocalConnection3D, or a layer of ann_to_snn's kinds
 static bool has_pool(const snn_net_t *net) {
     for (int c = 0; c < net->n_conns; ++c)
         if (net->conns[c].kind == SNN_CONN_MAXPOOL2D || net->conns[c].kind == SNN_CONN_LOCAL2D || net->conns[c].kind == SNN_CONN_CONV3D ||
-            net->conns[c].kind == SNN_CONN_CONV1D)
+            net->conns[c].kind == SNN_CONN_CONV1D || net->conns[c].kind == SNN_CONN_LOCAL3D)
             return true;
     for (int l = 0; l < net->n_layers; ++l)
         if (net->layers[l].kind == SNN_NODE_SUBIF || net->layers[l].kind == SNN_NODE_PASSTHROUGH) return true;
@@ -179,7 +184,8 @@ static bool has_syn(const snn_net_t *net) {
 static bool layer_needs_xpub(const snn_net_t *net, int l) {
     for (int c = 0; c < net->n_conns; ++c)
         if (net->conns[c].src == l && SNN_RULE_IS_STDP(net->conns[c].rule) && net->conns[c].kind != SNN_CONN_CONV2D &&
-            net->conns[c].kind != SNN_CONN_LOCAL2D && net->conns[c].kind != SNN_CONN_CONV3D && net->conns[c].kind != SNN_CONN_CONV1D)
+            net->conns[c].kind != SNN_CONN_LOCAL2D && net->conns[c].kind != SNN_CONN_CONV3D && net->conns[c].kind != SNN_CONN_CONV1D &&
+            net->conns[c].kind != SNN_CONN_LOCAL3D)
             return true;
     return false;
 }
@@ -215,7 +221,7 @@ static size_t layout_generic(const snn_net_t *net, const snn_run_opts_t *o, char
         for (int c = 0; c < net->n_conns; ++c)
             if (net->conns[c].src == l && net->conns[c].kind != SNN_CONN_CONV2D && net->conns[c].kind != SNN_CONN_MAXPOOL2D &&
                 net->conns[c].kind != SNN_CONN_LOCAL2D && net->conns[c].kind != SNN_CONN_CONV3D && net->conns[c].kind != SNN_CONN_CONV1D &&
-                nw > 32)
+                net->conns[c].kind != SNN_CONN_LOCAL3D && nw > 32)
                 wide_src = true;
         if (N) N->layers[l].anyf = wide_src ? (uint32_t *)(ws + off) : nullptr;
         if (wide_src) off += align_up(sizeof(uint32_t) * 3 * B);
@@ -275,7 +281,8 @@ int snn_b200_last_launch_count(void) { return g_last_launches; }
 static int select_tier(const snn_net_t *net, const snn_run_opts_t *opts, bool pn) {
     if (validate(net, opts) != SNN_OK) return 0;
     // one extra instantiation of the generic kernel each for sparse, feature and pooling plans (pooling: also plans with
-    // a LocalConnection2D, a Conv3dConnection, a Conv1dConnection, SubtractiveResetIFNodes or PassThroughNodes), not
+    // a LocalConnection2D, a LocalConnection3D, a Conv3dConnection, a Conv1dConnection, SubtractiveResetIFNodes or
+    // PassThroughNodes), not
     // combinations
     // (and one for plans with per-synapse bounds or rates)
     if ((int)has_sparse(net) + (int)has_feat(net) + (int)has_pool(net) + (int)has_syn(net) > 1) return 0;

@@ -98,8 +98,8 @@ struct DevNet {
     DevSparse sp[SNN_MAX_CONNS];
     int32_t any_feat;             // some MCC connection carries Probability / Mask / Intensity features
     int32_t any_pool;             // some connection is a MaxPool2dConnection (SNN_CONN_MAXPOOL2D), a LocalConnection2D
-                                  // (SNN_CONN_LOCAL2D), a Conv3dConnection (SNN_CONN_CONV3D) or a Conv1dConnection
-                                  // (SNN_CONN_CONV1D), or some layer is an SNN_NODE_SUBIF / SNN_NODE_PASSTHROUGH one: the
+                                  // (SNN_CONN_LOCAL2D), a Conv3dConnection (SNN_CONN_CONV3D), a Conv1dConnection
+                                  // (SNN_CONN_CONV1D) or a LocalConnection3D (SNN_CONN_LOCAL3D), or some layer is an SNN_NODE_SUBIF / SNN_NODE_PASSTHROUGH one: the
                                   // plan runs the POOL instantiation
     float *pool_r1[SNN_MAX_CONNS];   // MaxPool2dConnection: the workspace slot of its rates (pool_rate_slot)
 };
@@ -138,6 +138,23 @@ static inline int snn_local2d_geometry_ok(const snn_conn_t &C, int n_src, int n_
     if (C.hout != (C.hin - C.kh) / C.sh + 1 || C.wout != (C.win - C.kw) / C.sw + 1) return SNN_ERR_BAD_ARG;
     if ((long long)C.cin * C.hin * C.win != n_src || (long long)C.cout * C.hout * C.wout != n_tgt) return SNN_ERR_BAD_ARG;
     return SNN_OK;
+}
+
+// A LocalConnection3D's geometry (snn_b200.h): snn_local2d_geometry_ok on three axes, the depth axis in the fields
+// SNN_CONN_CONV3D uses.
+static inline int snn_local3d_geometry_ok(const snn_conn_t &C, int n_src, int n_tgt) {
+    if (!C.w || C.b) return SNN_ERR_BAD_ARG;
+    if (C.cin < 1 || C.cout < 1 || C.kd < 1 || C.kh < 1 || C.kw < 1 || C.sd < 1 || C.sh < 1 || C.sw < 1) return SNN_ERR_BAD_ARG;
+    if (C.pd != 0 || C.ph != 0 || C.pw != 0 || C.dh != 1 || C.dw != 1) return SNN_ERR_BAD_ARG;
+    if (C.kd > C.din || C.kh > C.hin || C.kw > C.win) return SNN_ERR_BAD_ARG;
+    if (C.dout != (C.din - C.kd) / C.sd + 1 || C.hout != (C.hin - C.kh) / C.sh + 1 || C.wout != (C.win - C.kw) / C.sw + 1)
+        return SNN_ERR_BAD_ARG;
+    if ((long long)C.cin * C.din * C.hin * C.win != n_src || (long long)C.cout * C.dout * C.hout * C.wout != n_tgt) return SNN_ERR_BAD_ARG;
+    return SNN_OK;
+}
+static inline bool snn_local_rule_ok(const snn_conn_t &C) {
+    return C.rule == SNN_RULE_NONE || C.rule == SNN_RULE_NOOP || C.rule == SNN_RULE_POSTPRE || C.rule == SNN_RULE_WDEP_POSTPRE ||
+           C.rule == SNN_RULE_HEBBIAN;
 }
 
 // A Conv3dConnection's geometry (snn_b200.h): the layer sizes, every output size (in - k + 2p) / s + 1 of a kernel that

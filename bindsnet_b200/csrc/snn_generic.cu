@@ -1,6 +1,6 @@
 // snn_generic.cu — generic persistent window kernel (any topology of Input / McCullochPitts / IF / LIF / BoostedLIF /
 // CurrentLIF / DiehlAndCook / SubtractiveResetIF / PassThrough populations joined by dense, convolutional, sparse,
-// pooling and 2-D locally connected connections).
+// pooling and 2-D and 3-D locally connected connections).
 //
 // One cooperative grid iterates the whole T-step window of Network.run (reference:
 // bindsnet/network/network.py:380-465) with at most four grid barriers per step and no host involvement.
@@ -53,10 +53,10 @@ __device__ __forceinline__ void sparse_unit(const DevNet &N, int u, int &c, int 
 // code (and register allocation) is exactly what it is without the feature.
 // FEAT: the plan holds a MulticompartmentConnection with Probability / Mask / Intensity features (snn_b200.h); only the
 // dense gather of phase 1 differs.  The two are not combined in one plan.
-// POOL: the plan holds a MaxPool2dConnection, a LocalConnection2D, a Conv3dConnection, a Conv1dConnection or a layer of
-// ann_to_snn's kinds (SNN_NODE_SUBIF, SNN_NODE_PASSTHROUGH, whose s is float32): phase 1 gathers the pooled spikes, the
-// local receptive fields and the 3-D and 1-D convolutions and steps those layers, the learning phase runs the local and
-// Conv1d rules and the Conv3d decay over the grid, normalize() scales the local rows and the 3-D and 1-D filters, and every
+// POOL: the plan holds a MaxPool2dConnection, a LocalConnection2D, a LocalConnection3D, a Conv3dConnection, a
+// Conv1dConnection or a layer of ann_to_snn's kinds (SNN_NODE_SUBIF, SNN_NODE_PASSTHROUGH, whose s is float32): phase 1
+// gathers the pooled spikes, the 2-D and 3-D local receptive fields and the 3-D and 1-D convolutions and steps those
+// layers, the learning phase runs the local and Conv1d rules and the Conv3d decay over the grid, normalize() scales the local rows and the 3-D and 1-D filters, and every
 // finalised spike of a pooling source advances its rates (pool_rate_step); the prologue writes the rates of step 0.  Not
 // combined with SPARSE or FEAT.  The
 // barriers are those of the plain window: the rates a gather reads were written before the barrier that ends the previous
@@ -204,6 +204,7 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                 if (POOL && N.conns[c].kind == SNN_CONN_LOCAL2D && N.conns[c].rule != SNN_RULE_NONE) phase3_local2d(N, c, blockIdx.x, G, t);
                 if (POOL && N.conns[c].kind == SNN_CONN_CONV3D && N.conns[c].rule != SNN_RULE_NONE) phase3_conv3d(N.conns[c], blockIdx.x, G);
                 if (POOL && N.conns[c].kind == SNN_CONN_CONV1D && N.conns[c].rule != SNN_RULE_NONE) phase3_conv1d(N, c, blockIdx.x, G, t);
+                if (POOL && N.conns[c].kind == SNN_CONN_LOCAL3D && N.conns[c].rule != SNN_RULE_NONE) phase3_local3d(N, c, blockIdx.x, G, t);
                 if (SPARSE && N.conns[c].kind == SNN_CONN_SPARSE) decay_sparse(N.conns[c], blockIdx.x, G);
             }
             GPROF(5)
@@ -247,7 +248,10 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                         normalize_conv_item(N.conns[c], N.conns[c].kd * N.conns[c].kh * N.conns[c].kw, tile, N.layers[li].nw);
                     else if (POOL && N.conns[c].kind == SNN_CONN_CONV1D) normalize_conv_item(N.conns[c], N.conns[c].kw, tile, N.layers[li].nw);
                     else if (POOL && N.conns[c].kind == SNN_CONN_LOCAL2D)
-                        normalize_local2d_item(N.conns[c], N.conns[c].cin * N.layers[li].L.n, tile, N.layers[li].nw);
+                        normalize_local2d_item(N.conns[c], N.conns[c].cin * N.layers[li].L.n, N.conns[c].kh * N.conns[c].kw, tile, N.layers[li].nw);
+                    else if (POOL && N.conns[c].kind == SNN_CONN_LOCAL3D)
+                        normalize_local2d_item(N.conns[c], N.conns[c].cin * N.layers[li].L.n, N.conns[c].kd * N.conns[c].kh * N.conns[c].kw, tile,
+                                             N.layers[li].nw);
                     else normalize_tile(N.conns[c], N.layers[N.conns[c].src].L.n, N.layers[li].L.n, tile, M.red);
                 }
         }
@@ -282,7 +286,7 @@ static int plan_units(DevNet &N, int cap) {
         N.p3_first[c] = p3;
         N.p3_rc[c] = 0;
         if (!N.learning || C.rule == SNN_RULE_NONE || C.kind == SNN_CONN_CONV2D || C.kind == SNN_CONN_SPARSE || C.kind == SNN_CONN_MAXPOOL2D ||
-            C.kind == SNN_CONN_LOCAL2D || C.kind == SNN_CONN_CONV3D || C.kind == SNN_CONN_CONV1D)
+            C.kind == SNN_CONN_LOCAL2D || C.kind == SNN_CONN_CONV3D || C.kind == SNN_CONN_CONV1D || C.kind == SNN_CONN_LOCAL3D)
             continue;   // (a MaxPool2dConnection has no weights to update; conv and local rules are spread over the grid)
         const int nwS = N.layers[C.src].nw, nwT = N.layers[C.tgt].nw;
         if (SNN_RULE_IS_MSTDP(C.rule)) { N.p3_rc[c] = 1; p3 += nwS; continue; }
@@ -308,7 +312,7 @@ static int plan_units(DevNet &N, int cap) {
     bool conv_rule = false;
     for (int c = 0; c < N.n_conns; ++c)
         if (N.learning && (N.conns[c].kind == SNN_CONN_CONV2D || N.conns[c].kind == SNN_CONN_LOCAL2D || N.conns[c].kind == SNN_CONN_CONV3D ||
-                           N.conns[c].kind == SNN_CONN_CONV1D) &&
+                           N.conns[c].kind == SNN_CONN_CONV1D || N.conns[c].kind == SNN_CONN_LOCAL3D) &&
             N.conns[c].rule != SNN_RULE_NONE)
             conv_rule = true;
     int grid = conv_rule ? cap : (int)(units < cap ? units : cap);

@@ -212,11 +212,44 @@ __global__ void __launch_bounds__(256) local2d_compute_kernel(snn_conn_t C, int 
 }
 
 __global__ void __launch_bounds__(SNN_GEN_THREADS) local2d_normalize_kernel(snn_conn_t C, int rows) {
-    normalize_local2d_item(C, rows, blockIdx.x, gridDim.x);
+    normalize_local2d_item(C, rows, C.kh * C.kw, blockIdx.x, gridDim.x);
 }
 
 __global__ void __launch_bounds__(SNN_GEN_THREADS) local2d_update_kernel(const __grid_constant__ DevNet N, int ci) {
     phase3_local2d(N, ci, blockIdx.x, gridDim.x, 0);
+}
+
+// LocalConnection3D.compute (topology.py:1866-1896) on byte spikes: the window gather's gather_local2d<.., true> order (k
+// ascending within a channel from +0, then the channels).  Thread = one target neuron of one sample.
+__global__ void __launch_bounds__(256) local3d_compute_kernel(snn_conn_t C, int ns, int nt, int B, const uint8_t *__restrict__ s,
+                                                              float *__restrict__ out) {
+    const size_t total = (size_t)B * nt;
+    const int K = C.kd * C.kh * C.kw, HW = C.hout * C.wout, P = C.dout * HW;
+    for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+        const int b = (int)(e / nt), j = (int)(e - (size_t)b * nt), l = j % P, oz = l / HW, r = l - oz * HW;
+        const int oy = r / C.wout, ox = r - oy * C.wout;
+        const uint8_t *sb = s + (size_t)b * ns;
+        float p = 0.0f;
+        for (int ci = 0; ci < C.cin; ++ci) {
+            const float *wr = C.w + ((size_t)ci * nt + j) * K;
+            float q = 0.0f;
+            for (int kz = 0; kz < C.kd; ++kz)
+                for (int ky = 0; ky < C.kh; ++ky)
+                    for (int kx = 0; kx < C.kw; ++kx)
+                        if (sb[((ci * C.din + oz * C.sd + kz) * C.hin + oy * C.sh + ky) * C.win + ox * C.sw + kx])
+                            q = q + wr[(kz * C.kh + ky) * C.kw + kx];
+            p = p + q;
+        }
+        out[e] = p;
+    }
+}
+
+__global__ void __launch_bounds__(SNN_GEN_THREADS) local3d_normalize_kernel(snn_conn_t C, int rows) {
+    normalize_local2d_item(C, rows, C.kd * C.kh * C.kw, blockIdx.x, gridDim.x);
+}
+
+__global__ void __launch_bounds__(SNN_GEN_THREADS) local3d_update_kernel(const __grid_constant__ DevNet N, int ci) {
+    phase3_local3d(N, ci, blockIdx.x, gridDim.x, 0);
 }
 
 // bit-pack the CURRENT spikes of the two layers of a connection into slot 0 (F32: a PassThroughNodes layer's float32 s)
@@ -320,6 +353,14 @@ int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, 
         SNN_LAUNCH(local2d_compute_kernel, blocks, 256, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
         return cuda_rc(cudaGetLastError());
     }
+    if (conn->kind == SNN_CONN_LOCAL3D) {
+        const int rc = snn_local3d_geometry_ok(*conn, n_src, n_tgt);
+        if (rc != SNN_OK) return rc;
+        const size_t total = (size_t)B * n_tgt;
+        const int blocks = (int)((total + 255) / 256 < 4736 ? (total + 255) / 256 : 4736);
+        SNN_LAUNCH(local3d_compute_kernel, blocks, 256, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
+        return cuda_rc(cudaGetLastError());
+    }
     if (conn->kind == SNN_CONN_CONV3D) {
         const int rc = snn_conv3d_geometry_ok(*conn, n_src, n_tgt);
         if (rc != SNN_OK) return rc;
@@ -383,10 +424,16 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
     }
     const bool pass = net->layers[C.src].kind == SNN_NODE_PASSTHROUGH || net->layers[C.tgt].kind == SNN_NODE_PASSTHROUGH;
     if (pass && C.rule != SNN_RULE_NONE && C.rule != SNN_RULE_NOOP) return SNN_ERR_UNSUPPORTED;   // (snn_b200.h)
-    // the single-operator update is the dense [n_src, n_tgt] rule application or a LocalConnection2D's; convolutional
-    // weights and the reward-modulated rules (whose state lives in the window plan) are only updated inside run_window
-    const bool local = C.kind == SNN_CONN_LOCAL2D, conv1d = C.kind == SNN_CONN_CONV1D;
-    if (C.kind != SNN_CONN_DENSE && C.kind != SNN_CONN_MCC && !local && !conv1d) return SNN_ERR_UNSUPPORTED;
+    // the single-operator update is the dense [n_src, n_tgt] rule application or a LocalConnection2D's / 3D's or
+    // Conv1dConnection's; other convolutional weights and the reward-modulated rules (whose state lives in the window
+    // plan) are only updated inside run_window
+    const bool local = C.kind == SNN_CONN_LOCAL2D, conv1d = C.kind == SNN_CONN_CONV1D, local3d = C.kind == SNN_CONN_LOCAL3D;
+    if (C.kind != SNN_CONN_DENSE && C.kind != SNN_CONN_MCC && !local && !conv1d && !local3d) return SNN_ERR_UNSUPPORTED;
+    if (local3d) {
+        const int rc = snn_local3d_geometry_ok(C, net->layers[C.src].n, net->layers[C.tgt].n);
+        if (rc != SNN_OK) return rc;
+        if (!snn_local_rule_ok(C) || C.mask) return SNN_ERR_UNSUPPORTED;
+    }
     if (local) {
         const int rc = snn_local2d_geometry_ok(C, net->layers[C.src].n, net->layers[C.tgt].n);
         if (rc != SNN_OK) return rc;
@@ -431,6 +478,12 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
         SNN_LAUNCH(local2d_update_kernel, blocks, SNN_GEN_THREADS, 0, stream, N, ci);
         return cuda_rc(cudaGetLastError());
     }
+    if (local3d) {   // one warp per row segment, like the window's learning phase
+        const size_t units = (size_t)N.layers[C.tgt].L.n * ((C.cin * C.kd * C.kh * C.kw + 32 * SNN_LOCAL3D_EPL - 1) / (32 * SNN_LOCAL3D_EPL));
+        const int blocks = (int)((units + SNN_GEN_WARPS - 1) / SNN_GEN_WARPS < 1184 ? (units + SNN_GEN_WARPS - 1) / SNN_GEN_WARPS : 1184);
+        SNN_LAUNCH(local3d_update_kernel, blocks, SNN_GEN_THREADS, 0, stream, N, ci);
+        return cuda_rc(cudaGetLastError());
+    }
     if (conv1d) {   // one warp per group of elements, like the window's learning phase
         const size_t NW = (size_t)C.cout * C.cin * C.kw;
         const int blocks = (int)((NW + SNN_GEN_WARPS - 1) / SNN_GEN_WARPS < 1184 ? (NW + SNN_GEN_WARPS - 1) / SNN_GEN_WARPS : 1184);
@@ -456,6 +509,11 @@ int snn_b200_conn_normalize(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt
     if (conn->kind == SNN_CONN_LOCAL2D) {   // rows of w viewed as [cin * n_tgt, K]
         const int rows = conn->cin * n_tgt;
         SNN_LAUNCH(local2d_normalize_kernel, (rows + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, rows);
+        return cuda_rc(cudaGetLastError());
+    }
+    if (conn->kind == SNN_CONN_LOCAL3D) {   // rows of w viewed as [cin * n_tgt, K]
+        const int rows = conn->cin * n_tgt;
+        SNN_LAUNCH(local3d_normalize_kernel, (rows + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, rows);
         return cuda_rc(cudaGetLastError());
     }
     if (conn->kind == SNN_CONN_CONV2D) {

@@ -444,28 +444,35 @@ __device__ __forceinline__ float gather_conv1d(const snn_conn_t &C, const uint32
 // the bit row 32 at a time, as in gather_conv.  The weights are read where they are: a lane walks its own contiguous row
 // w[ci, j, :] (K floats), so the set bits of one row land in the same 32-byte sectors.  A weight under a silent input is
 // never read, which differs from the reference's s_unfold * w for a non-finite weight (DESIGN.md section 8).
-template <bool STAGED_BITS>
+// D3: LocalConnection3D.compute (topology.py:1866-1896), j = (f, oz, oy, ox), the same sums with the kernel rows
+// (ci, kz, ky) of the depth axis (din / kd / sd / dout, snn_b200.h SNN_CONN_LOCAL3D); without it the depth term is 1 and
+// the depth fields, which a LocalConnection2D leaves as the sparse storage, are never read.
+template <bool STAGED_BITS, bool D3 = false>
 __device__ __forceinline__ float gather_local2d(const snn_conn_t &C, const uint32_t *sb, int n, int j, bool valid) {
     if (!valid) return 0.0f;
-    const int K = C.kh * C.kw, P = C.hout * C.wout, l = j % P, oy = l / C.wout, ox = l - oy * C.wout;
+    const int kd = D3 ? C.kd : 1, din = D3 ? C.din : 1, HW = C.hout * C.wout;
+    const int K = kd * C.kh * C.kw, P = (D3 ? C.dout : 1) * HW, l = j % P;
+    const int oz = D3 ? l / HW : 0, r = l - oz * HW, oy = r / C.wout, ox = r - oy * C.wout;
     float p = 0.0f;
     for (int ci = 0; ci < C.cin; ++ci) {
         const float *wr = C.w + ((size_t)ci * n + j) * K;
         float q = 0.0f;
-        for (int ky = 0; ky < C.kh; ++ky) {
-            const int row = (ci * C.hin + oy * C.sh + ky) * C.win + ox * C.sw;
-            for (int kx0 = 0; kx0 < C.kw; kx0 += 32) {
-                const int cnt = min(32, C.kw - kx0), bit0 = row + kx0, w0 = bit0 >> 5, sft = bit0 & 31;
-                const uint32_t lo = STAGED_BITS ? sb[w0] : __ldcg(sb + w0);
-                const uint32_t hi = sft + cnt > 32 ? (STAGED_BITS ? sb[w0 + 1] : __ldcg(sb + w0 + 1)) : 0u;
-                uint32_t bits = __funnelshift_r(lo, hi, sft) & (cnt >= 32 ? 0xffffffffu : ((1u << cnt) - 1u));
-                while (bits) {
-                    const int k = ky * C.kw + kx0 + __ffs(bits) - 1;
-                    bits &= bits - 1;
-                    q = q + __ldcg(wr + k);
+        for (int kz = 0; kz < kd; ++kz)
+            for (int ky = 0; ky < C.kh; ++ky) {
+                const int row = ((ci * din + (D3 ? oz * C.sd + kz : 0)) * C.hin + oy * C.sh + ky) * C.win + ox * C.sw;
+                const int krow = (kz * C.kh + ky) * C.kw;
+                for (int kx0 = 0; kx0 < C.kw; kx0 += 32) {
+                    const int cnt = min(32, C.kw - kx0), bit0 = row + kx0, w0 = bit0 >> 5, sft = bit0 & 31;
+                    const uint32_t lo = STAGED_BITS ? sb[w0] : __ldcg(sb + w0);
+                    const uint32_t hi = sft + cnt > 32 ? (STAGED_BITS ? sb[w0 + 1] : __ldcg(sb + w0 + 1)) : 0u;
+                    uint32_t bits = __funnelshift_r(lo, hi, sft) & (cnt >= 32 ? 0xffffffffu : ((1u << cnt) - 1u));
+                    while (bits) {
+                        const int k = krow + kx0 + __ffs(bits) - 1;
+                        bits &= bits - 1;
+                        q = q + __ldcg(wr + k);
+                    }
                 }
             }
-        }
         p = p + q;
     }
     return p;
@@ -621,15 +628,16 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
 
     // a convolutional input: stage the chunk's source bit rows and the taps of this tile's output channels (POOL: a
     // Conv3dConnection input likewise, with the depth axis in its channel size and taps; a Conv1dConnection input too,
-    // its height axis 1; a LocalConnection2D input gets its bit rows staged the same way, its weights are per target,
-    // not taps)
+    // its height axis 1; a LocalConnection2D or LocalConnection3D input gets its bit rows staged the same way, its
+    // weights are per target, not taps)
     int conv_c = -1, conv_slot = 0, co_base = 0;
     bool st_bits = false, st_taps = false;
     ConvGeo geo = {};
     for (int c = 0; c < N.n_conns && conv_c < 0; ++c)
         if (N.conns[c].tgt == li &&
             (N.conns[c].kind == SNN_CONN_CONV2D ||
-             (POOL && (N.conns[c].kind == SNN_CONN_LOCAL2D || N.conns[c].kind == SNN_CONN_CONV3D || N.conns[c].kind == SNN_CONN_CONV1D))))
+             (POOL && (N.conns[c].kind == SNN_CONN_LOCAL2D || N.conns[c].kind == SNN_CONN_CONV3D || N.conns[c].kind == SNN_CONN_CONV1D ||
+                      N.conns[c].kind == SNN_CONN_LOCAL3D))))
             conv_c = c;
     if (conv_c >= 0) {
         const snn_conn_t &C = N.conns[conv_c];
@@ -643,7 +651,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
         co_base = (tile * SNN_TILE) / Lhw;
         const int co_hi = min(n - 1, tile * SNN_TILE + SNN_TILE - 1) / Lhw;
         const int ntaps = (co_hi - co_base + 1) * K;
-        st_taps = ntaps <= SNN_CONV_STAGE_TAPS && (!POOL || C.kind != SNN_CONN_LOCAL2D);
+        st_taps = ntaps <= SNN_CONV_STAGE_TAPS && (!POOL || (C.kind != SNN_CONN_LOCAL2D && C.kind != SNN_CONN_LOCAL3D));
         if (st_bits) {
             const uint32_t *src = S.bits + ((size_t)conv_slot * B + b0) * S.nw;
             for (int k0 = threadIdx.x; k0 < words; k0 += 4 * SNN_GEN_THREADS) {
@@ -680,7 +688,8 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
             fwn[q] = 0u; afn[q] = 1u;
             if (q < ncl && b < b1 && N.conns[cl[q]].kind != SNN_CONN_CONV2D && !(SPARSE && N.conns[cl[q]].kind == SNN_CONN_SPARSE) &&
                 !(POOL && (N.conns[cl[q]].kind == SNN_CONN_MAXPOOL2D || N.conns[cl[q]].kind == SNN_CONN_LOCAL2D ||
-                           N.conns[cl[q]].kind == SNN_CONN_CONV3D || N.conns[cl[q]].kind == SNN_CONN_CONV1D))) {
+                           N.conns[cl[q]].kind == SNN_CONN_CONV3D || N.conns[cl[q]].kind == SNN_CONN_CONV1D ||
+                           N.conns[cl[q]].kind == SNN_CONN_LOCAL3D))) {
                 const snn_conn_t &C = N.conns[cl[q]];
                 const DevLayer &S = N.layers[C.src];
                 const int slot = (N.one_step && C.src < li) ? wr : rd;
@@ -760,6 +769,9 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
             } else if (POOL && C.kind == SNN_CONN_LOCAL2D) {
                 p = c == conv_c && st_bits ? gather_local2d<true>(C, M.cbits + (size_t)(b - b0) * S.nw, n, j, valid)
                                            : gather_local2d<false>(C, S.bits + ((size_t)slot * B + b) * S.nw, n, j, valid);
+            } else if (POOL && C.kind == SNN_CONN_LOCAL3D) {
+                p = c == conv_c && st_bits ? gather_local2d<true, true>(C, M.cbits + (size_t)(b - b0) * S.nw, n, j, valid)
+                                           : gather_local2d<false, true>(C, S.bits + ((size_t)slot * B + b) * S.nw, n, j, valid);
             } else if (SPARSE && C.kind == SNN_CONN_SPARSE) {   // gathered by phase_sparse ahead of this phase
                 p = valid ? __ldcg(N.sp[c].out + (size_t)b * n + j) : 0.0f;
                 if (C.b && valid) p = p + C.b[j];
@@ -1334,12 +1346,15 @@ __device__ __forceinline__ float stdp_rule_apply(const snn_conn_t &C, float x, f
 }
 
 // The source neuron of element (n', m) of a LocalConnection2D rule (snn_b200.h): the unfolded source at flat position
-// (n' % P) * cin * K + m in [cin, P, K] order.
+// (n' % P) * cin * K + m in [cin, P, K] order.  D3: a LocalConnection3D's (P and K over the depth axis too); without it the
+// depth term is 1 and the depth fields are never read.
+template <bool D3 = false>
 __host__ __device__ __forceinline__ int local2d_rule_source(const snn_conn_t &C, int n, int m) {
-    const int K = C.kh * C.kw, P = C.hout * C.wout;
+    const int HW = C.hout * C.wout, KHW = C.kh * C.kw, K = (D3 ? C.kd : 1) * KHW, P = (D3 ? C.dout : 1) * HW;
     const int q = (n % P) * C.cin * K + m, ci = q / (P * K), r = q - ci * P * K, l = r / K, k = r - l * K;
-    const int oy = l / C.wout, ox = l - oy * C.wout, ky = k / C.kw, kx = k - ky * C.kw;
-    return (ci * C.hin + oy * C.sh + ky) * C.win + ox * C.sw + kx;
+    const int oz = D3 ? l / HW : 0, lr = l - oz * HW, kz = D3 ? k / KHW : 0, kr = k - kz * KHW;
+    const int oy = lr / C.wout, ox = lr - oy * C.wout, ky = kr / C.kw, kx = kr - ky * C.kw;
+    return ((ci * (D3 ? C.din : 1) + (D3 ? oz * C.sd + kz : 0)) * C.hin + oy * C.sh + ky) * C.win + ox * C.sw + kx;
 }
 
 // PostPre / WeightDependentPostPre / Hebbian on a LocalConnection2D (learning.py:258-320, 717-791, 1186-1250), and the
@@ -1370,6 +1385,80 @@ __device__ void phase3_local2d(const DevNet &N, int ci_, int cta, int ncta, int 
         }
         if (C.reduction == SNN_REDUCE_MEAN) { U = U / (float)B; V = V / (float)B; }
         C.w[e] = stdp_rule_apply(C, __ldcg(C.w + e), U, V, pre_on, post_on);
+    }
+}
+
+// PostPre / WeightDependentPostPre / Hebbian on a LocalConnection3D (learning.py:322-388, 793-871, 1249-1314), and the
+// decay of learning.NoOp.  Element (n', m) of w (flat n' * cin * K + m, source src = local2d_rule_source<true>) takes
+//   U = reduce_b x_tgt[b, n'] * s_src[b, src],  V = reduce_b s_tgt[b, n'] * x_src[b, src]
+// with the samples in ascending b from +0 and the terms of silent spikes skipped, as phase3_local2d.  Organised by target
+// row rather than by element: a unit is one warp over SNN_LOCAL3D_EPL * 32 consecutive m of one row n', lane l holding
+// m0 + 32 i + l.  x_tgt[b, n'] and s_tgt[b, n'] are then warp-uniform: the warp loads them for 32 samples at a time, and
+// a sample whose x_tgt is zero (its U terms are +-0, which leave the +0-started sum as it is) or whose target is silent
+// is skipped by the whole warp for U or V.  For cin = 1 neighbouring lanes read neighbouring source bits and traces.
+// Traces are read from the layers' own arrays, framed by the grid barriers around the learning phase.
+#define SNN_LOCAL3D_EPL 4
+__device__ void phase3_local3d(const DevNet &N, int ci_, int cta, int ncta, int t) {
+    const snn_conn_t &C = N.conns[ci_];
+    const DevLayer &S = N.layers[C.src], &G = N.layers[C.tgt];
+    const int B = N.B, ns = S.L.n, nt = G.L.n, Mw = C.cin * C.kd * C.kh * C.kw;
+    if (!SNN_RULE_IS_STDP(C.rule)) {   // learning.NoOp: w *= weight_decay (learning.py:93-94), no clamp
+        const size_t NW = (size_t)nt * Mw;
+        if (C.weight_decay != 0.0f)
+            for (size_t e = (size_t)cta * SNN_GEN_THREADS + threadIdx.x; e < NW; e += (size_t)ncta * SNN_GEN_THREADS)
+                C.w[e] = __ldcg(C.w + e) * C.weight_decay;
+        return;
+    }
+    const bool hebb = C.rule == SNN_RULE_HEBBIAN;
+    const bool pre_on = C.nu0 != 0.0f || hebb, post_on = C.nu1 != 0.0f || hebb;
+    const int wr = t & 1, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int segs = (Mw + 32 * SNN_LOCAL3D_EPL - 1) / (32 * SNN_LOCAL3D_EPL);
+    const long long units = (long long)nt * segs;
+    for (long long u = (long long)cta * SNN_GEN_WARPS + warp; u < units; u += (long long)ncta * SNN_GEN_WARPS) {
+        const int n = (int)(u / segs), m0 = (int)(u - (long long)n * segs) * 32 * SNN_LOCAL3D_EPL + lane;
+        int src[SNN_LOCAL3D_EPL];
+        float U[SNN_LOCAL3D_EPL], V[SNN_LOCAL3D_EPL];
+        #pragma unroll
+        for (int i = 0; i < SNN_LOCAL3D_EPL; ++i) {
+            const int m = m0 + 32 * i;
+            src[i] = m < Mw ? local2d_rule_source<true>(C, n, m) : -1;
+            U[i] = 0.0f; V[i] = 0.0f;
+        }
+        for (int b0 = 0; b0 < B; b0 += 32) {
+            const int b = b0 + lane;
+            float xt = 0.0f;
+            bool st = false;
+            if (b < B) {
+                if (pre_on) xt = __ldcg(G.L.x + (size_t)b * nt + n);
+                if (post_on) st = bit_of(G.bits + ((size_t)wr * B + b) * G.nw, n);
+            }
+            uint32_t um = __ballot_sync(0xffffffffu, xt != 0.0f), vm = __ballot_sync(0xffffffffu, st);
+            while (um) {   // samples ascending
+                const int q = __ffs(um) - 1;
+                um &= um - 1;
+                const float xb = __shfl_sync(0xffffffffu, xt, q);
+                const uint32_t *sb = S.bits + ((size_t)wr * B + b0 + q) * S.nw;
+                #pragma unroll
+                for (int i = 0; i < SNN_LOCAL3D_EPL; ++i)
+                    if (src[i] >= 0 && bit_of(sb, src[i])) U[i] = U[i] + xb;
+            }
+            while (vm) {
+                const int q = __ffs(vm) - 1;
+                vm &= vm - 1;
+                const float *xs = S.L.x + (size_t)(b0 + q) * ns;
+                #pragma unroll
+                for (int i = 0; i < SNN_LOCAL3D_EPL; ++i)
+                    if (src[i] >= 0) V[i] = V[i] + __ldcg(xs + src[i]);
+            }
+        }
+        #pragma unroll
+        for (int i = 0; i < SNN_LOCAL3D_EPL; ++i) {
+            if (src[i] < 0) continue;
+            float u1 = U[i], v1 = V[i];
+            if (C.reduction == SNN_REDUCE_MEAN) { u1 = u1 / (float)B; v1 = v1 / (float)B; }
+            const size_t e = (size_t)n * Mw + m0 + 32 * i;
+            C.w[e] = stdp_rule_apply(C, __ldcg(C.w + e), u1, v1, pre_on, post_on);
+        }
     }
 }
 
@@ -1749,11 +1838,10 @@ __device__ void normalize_conv_item(const snn_conn_t &C, int KK, int tile, int n
     }
 }
 
-// LocalConnection2D.normalize (topology.py:1748-1759): w viewed as [cin * n, K], every row scaled by norm / its sum (sum in
-// ascending k; `norm / sum` is torch's reciprocal(sum) * norm).  No guard against a zero sum, like the reference: such a row
-// becomes inf / NaN.
-__device__ void normalize_local2d_item(const snn_conn_t &C, int rows, int tile, int ntiles) {
-    const int K = C.kh * C.kw;
+// LocalConnection2D.normalize (topology.py:1748-1759) and LocalConnection3D.normalize (:1898-1909): w viewed as
+// [cin * n, K], every row scaled by norm / its sum (sum in ascending k; `norm / sum` is torch's reciprocal(sum) * norm).
+// No guard against a zero sum, like the reference: such a row becomes inf / NaN.
+__device__ void normalize_local2d_item(const snn_conn_t &C, int rows, int K, int tile, int ntiles) {
     for (int r = tile * SNN_GEN_THREADS + threadIdx.x; r < rows; r += ntiles * SNN_GEN_THREADS) {
         float *w = C.w + (size_t)r * K;
         float tot = 0.0f;

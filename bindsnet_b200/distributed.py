@@ -42,7 +42,7 @@ class ShardedWindowRunner:
         """Connections whose weights change inside a window (a learning rule, or the end-of-run normalize),
         with the constants the combine needs.  Built from the objects' attributes — not from the per-window
         plan, which reward-modulated rules can only fill during a run."""
-        from .network.topology import Conv1dConnection, Conv2dConnection, Conv3dConnection
+        from .network.topology import Conv1dConnection, Conv2dConnection, Conv3dConnection, LocalConnection3D
 
         out = []
         for conn in self.network.connections.values():
@@ -66,9 +66,10 @@ class ShardedWindowRunner:
                 d.has_clamp = int(code >= _abi.SNN_RULE_POSTPRE and (math.isfinite(d.wmin) or math.isfinite(d.wmax)))
             if d.rule >= _abi.SNN_RULE_POSTPRE or d.has_norm:
                 # [Cout,Cin,kh,kw] / [Cout,Cin,kd,kh,kw] / [Cout,Cin,k] weights normalise per filter (topology.py:824-837,
-                # 1004-1018, 665-676), the combine kernel per column of an [n_src,n_tgt] matrix: for them it applies sum +
-                # clamp only, the connection's own normalize follows
-                d._conv = isinstance(conn, (Conv1dConnection, Conv2dConnection, Conv3dConnection))
+                # 1004-1018, 665-676), a LocalConnection3D's [Cin,n,K] per contiguous row (:1898-1909), the combine kernel
+                # per column of an [n_src,n_tgt] matrix: for them it applies sum + clamp only, the connection's own
+                # normalize follows
+                d._conv = isinstance(conn, (Conv1dConnection, Conv2dConnection, Conv3dConnection, LocalConnection3D))
                 out.append((conn, d))
         return out
 

@@ -1,8 +1,8 @@
 """Learning rules for ``Connection`` — host-side mirror of ``bindsnet/learning/learning.py``
 (``LearningRule`` :25-104, ``NoOp`` :107-146, ``PostPre`` :149-420 / :457-497 (conv2d),
 ``WeightDependentPostPre`` :562-653 / :920-975, ``Hebbian`` :1052-1136 / :1348-1380, ``MSTDP``; the three unsupervised
-rules also on ``LocalConnection2D``, :258-320 / :717-791 / :1186-1250, and on ``Conv1dConnection``, :422-455 / :873-918 /
-:1316-1346; on ``Conv3dConnection`` only what the reference can run, see ``Conv3dConnection``).  The rule objects hold hyper-parameters; the update
+rules also on ``LocalConnection2D``, :258-320 / :717-791 / :1186-1250, on ``LocalConnection3D``, :322-388 / :793-871 /
+:1249-1314, and on ``Conv1dConnection``, :422-455 / :873-918 / :1316-1346; on ``Conv3dConnection`` only what the reference can run, see ``Conv3dConnection``).  The rule objects hold hyper-parameters; the update
 itself is fused into the CUDA window kernels (``Network.run``) or submitted for one step by
 ``rule.update()``."""
 from __future__ import annotations
@@ -111,10 +111,12 @@ def _check_connection(rule, connection) -> None:
     ignores dilation, so a dilated filter is refused.  On ``Conv3dConnection`` (``_conv3d_connection_update``) the
     post-synaptic-only form of PostPre / WeightDependentPostPre pairs the kernel axes transposed against ``w``
     (learning.py:517-530, 996-1010); it is not built, so such a rule is refused here.  ``Conv1dConnection``
-    (``_conv1d_connection_update``) runs all three."""
-    from ..network.topology import Connection, Conv1dConnection, Conv2dConnection, Conv3dConnection, LocalConnection2D
+    (``_conv1d_connection_update``) and ``LocalConnection3D`` (``_local_connection3d_update``) run all three."""
+    from ..network.topology import (Connection, Conv1dConnection, Conv2dConnection, Conv3dConnection, LocalConnection2D,
+                                    LocalConnection3D)
 
-    if not isinstance(connection, (Connection, Conv2dConnection, LocalConnection2D, Conv3dConnection, Conv1dConnection)):
+    if not isinstance(connection, (Connection, Conv2dConnection, LocalConnection2D, Conv3dConnection, Conv1dConnection,
+                                   LocalConnection3D)):
         raise NotImplementedError("This learning rule is not supported for this Connection type.")
     if isinstance(connection, Conv3dConnection) and isinstance(rule, (PostPre, WeightDependentPostPre)) and \
             float(rule.nu[0]) == 0.0 and float(rule.nu[1]) != 0.0:
@@ -187,8 +189,12 @@ class MSTDP(_RewardModulated, LearningRule):
 
     def __init__(self, connection, nu=None, reduction=None, weight_decay: float = 0.0, **kwargs) -> None:
         super().__init__(connection=connection, nu=nu, reduction=reduction, weight_decay=weight_decay, **kwargs)
-        from ..network.topology import Connection, Conv1dConnection, Conv2dConnection, Conv3dConnection
+        from ..network.topology import Connection, Conv1dConnection, Conv2dConnection, Conv3dConnection, LocalConnection3D
 
+        if isinstance(connection, LocalConnection3D):
+            # learning.py:1764-1866 / 2458-: the local forms of the reward-modulated rules are not built
+            raise NotImplementedError(f"{type(self).__name__} on a LocalConnection3D is not implemented: its local form "
+                                      "(learning.py:1764-1866) is not built on the CUDA core")
         if isinstance(connection, Conv1dConnection):
             # learning.py:1868-1940 / 2571-: at B > 1 the eligibility [B, out, in * k] is viewed into w's shape, which
             # fails; at B = 1 the rule sums the eligibility over the output channels from the second step on

@@ -99,7 +99,7 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
         conn._fill_desc(d, dt, rule)
         return
     conn._fill_desc(d, dt, rule)
-    if d.kind == _abi.SNN_CONN_LOCAL2D:   # [cin, n, K] weights, no bias (topology.py:1717-1740 never reads b)
+    if d.kind in (_abi.SNN_CONN_LOCAL2D, _abi.SNN_CONN_LOCAL3D):   # [cin, n, K] weights, no bias (compute never reads b)
         w = conn.w
         if w.dtype != torch.float32 or not w.is_contiguous():
             raise TypeError("connection weights must be contiguous float32")
@@ -319,11 +319,11 @@ def build_net(
         check_passthrough(net, i, type(conn).__name__)
     conns = [net.conns[i] for i in range(net.n_conns)]
     layers = [net.layers[i] for i in range(net.n_layers)]
-    pool_kinds = (_abi.SNN_CONN_MAXPOOL2D, _abi.SNN_CONN_LOCAL2D, _abi.SNN_CONN_CONV3D, _abi.SNN_CONN_CONV1D)
+    pool_kinds = (_abi.SNN_CONN_MAXPOOL2D, _abi.SNN_CONN_LOCAL2D, _abi.SNN_CONN_CONV3D, _abi.SNN_CONN_CONV1D, _abi.SNN_CONN_LOCAL3D)
     if (any(d.kind in pool_kinds for d in conns) or any(d.kind in CONVERSION_KINDS for d in layers)) and any(
             d.kind == _abi.SNN_CONN_SPARSE or d.f_prob or d.f_mask or d.f_int for d in conns):
         raise NotImplementedError("a network with a MaxPool2dConnection, LocalConnection2D, Conv3dConnection, Conv1dConnection, "
-                                  "SubtractiveResetIFNodes or PassThroughNodes and a SparseConnection or MulticompartmentConnection "
+                                  "LocalConnection3D, SubtractiveResetIFNodes or PassThroughNodes and a SparseConnection or MulticompartmentConnection "
                                   "features is not implemented by the CUDA core (each has its own instantiation of the window kernel)")
     check_neuron_params(layers, conns)
     return net, keep
@@ -335,12 +335,12 @@ def check_neuron_params(layers, conns) -> None:
     or pooling one."""
     if not any(d.kind & _abi.SNN_NODE_PN for d in layers):
         return
-    pool_kinds = (_abi.SNN_CONN_MAXPOOL2D, _abi.SNN_CONN_LOCAL2D, _abi.SNN_CONN_CONV3D, _abi.SNN_CONN_CONV1D)
+    pool_kinds = (_abi.SNN_CONN_MAXPOOL2D, _abi.SNN_CONN_LOCAL2D, _abi.SNN_CONN_CONV3D, _abi.SNN_CONN_CONV1D, _abi.SNN_CONN_LOCAL3D)
     if any(d.kind == _abi.SNN_CONN_SPARSE or d.kind in pool_kinds or (d.kind == _abi.SNN_CONN_MCC and (d.f_prob or d.f_mask or d.f_int))
            for d in conns) or any(d.kind in CONVERSION_KINDS for d in layers):
         raise NotImplementedError("per-neuron parameter tensors in a network with a SparseConnection, MulticompartmentConnection "
                                   "features, a MaxPool2dConnection, LocalConnection2D, Conv3dConnection, Conv1dConnection, "
-                                  "SubtractiveResetIFNodes or PassThroughNodes are not implemented by the CUDA core (each has its own instantiation of "
+                                  "LocalConnection3D, SubtractiveResetIFNodes or PassThroughNodes are not implemented by the CUDA core (each has its own instantiation of "
                                   "the window kernel)")
 
 

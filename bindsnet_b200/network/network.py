@@ -381,7 +381,8 @@ class Network(torch.nn.Module):
             if type(layer) not in builtin_nodes and (layer.kind is None or type(layer).forward is not N.Nodes.forward):
                 return True
         builtin_conns = (Tp.Connection, Tp.MulticompartmentConnection, Tp.Conv2dConnection, Tp.LocalConnection, Tp.SparseConnection,
-                         Tp.MaxPool2dConnection, Tp.LocalConnection2D, Tp.Conv3dConnection, Tp.Conv1dConnection)
+                         Tp.MaxPool2dConnection, Tp.LocalConnection2D, Tp.Conv3dConnection, Tp.Conv1dConnection,
+                         Tp.LocalConnection3D)
         for conn in self.connections.values():
             if type(conn) not in builtin_conns:
                 return True

@@ -468,6 +468,9 @@ def _triple(x):
     return tuple(x) if isinstance(x, (tuple, list)) else (x, x, x)
 
 
+_MISSING = object()   # a required argument of the reference that was not passed (LocalConnection3D)
+
+
 class Conv3dConnection(AbstractConnection):
     """3-D convolutional synapses (reference: topology.py:847-1025).  Source and target populations are
     ``[C, D, H, W]`` shaped; ``w`` is ``[out_channels, in_channels, kd, kh, kw]``, ``b`` ``[out_channels]`` (zeros by
@@ -1019,6 +1022,119 @@ class LocalConnection2D(AbstractConnection):
             self.update_rule._fill_desc(d)
 
 
+class LocalConnection3D(AbstractConnection):
+    """Three-dimensional locally connected synapses (reference: topology.py:1770-1917): every target neuron has weights of
+    its own over one ``kernel_size`` window of a ``[C, H, W, D]`` source, ``n_filters`` neurons per window.  ``w`` is
+    ``[in_channels, n_filters * conv_prod, kernel_prod]``; target neuron ``f * conv_prod + p`` sees window ``p``.  Inside
+    ``Network.run`` the generic window kernel gathers each target's receptive field from the source spikes and applies
+    ``PostPre``, ``WeightDependentPostPre``, ``Hebbian`` or ``NoOp``; ``normalize`` scales every ``kernel_prod`` row of
+    ``w`` to sum ``norm``.
+
+    As in the reference: ``w`` is drawn with ``torch.rand`` and clamped when a bound is finite; passing ``w=`` raises
+    ``AttributeError`` (the reference's shape check reads ``self.out_channels``, which it never sets); ``b`` is stored and
+    never used; a target with other than ``n_filters * conv_prod`` neurons, or a kernel larger than the source, raises
+    ``RuntimeError`` when the network runs (the reference fails in its first ``compute``); ``reset_state_variables`` also
+    resets the target layer.  The rules' update follows the reference's reshape of the unfolded source, which for
+    ``in_channels > 1`` pairs a weight with another source neuron than ``compute`` does (include/snn_b200.h,
+    SNN_CONN_LOCAL3D).  A source or target that is not a population with a ``[C, H, W, D]`` source shape raises
+    ``NotImplementedError`` before the other arguments are looked at, so such a call without ``stride`` / ``n_filters``
+    raises it where the reference raises ``TypeError`` (DESIGN.md section 8)."""
+
+    def __init__(self, source: Nodes, target: Nodes, kernel_size=_MISSING, stride=_MISSING, n_filters=_MISSING,
+                 nu: Optional[Union[float, Sequence[float], Sequence[torch.Tensor]]] = None, reduction: Optional[callable] = None,
+                 weight_decay: float = 0.0, w_dtype: torch.dtype = torch.float32, **kwargs) -> None:
+        for name, layer in (("source", source), ("target", target)):
+            if not isinstance(layer, Nodes) or (name == "source" and len(layer.shape) != 4):
+                shape = list(layer.shape) if isinstance(layer, Nodes) else type(layer).__name__
+                raise NotImplementedError(f"LocalConnection3D is built from a [C, H, W, D] source population into a population "
+                                          f"only; the {name} is {shape}")
+        missing = [n for n, v in (("kernel_size", kernel_size), ("stride", stride), ("n_filters", n_filters)) if v is _MISSING]
+        if missing:
+            names = " and ".join(f"'{n}'" for n in missing) if len(missing) < 3 else "'kernel_size', 'stride', and 'n_filters'"
+            raise TypeError(f"LocalConnection3D.__init__() missing {len(missing)} required positional argument"
+                            f"{'s' if len(missing) > 1 else ''}: {names}")
+        if w_dtype != torch.float32:
+            raise NotImplementedError("bindsnet_b200 computes in float32 only (SURVEY.md §8b)")
+        super().__init__(source, target, nu, reduction, weight_decay, **kwargs)
+        self.kernel_size, self.stride, self.n_filters = _triple(kernel_size), _triple(stride), n_filters
+        self.in_channels, input_height, input_width, input_depth = (source.shape[0], source.shape[1], source.shape[2],
+                                                                    source.shape[3])
+        height = int((input_height - self.kernel_size[0]) / self.stride[0]) + 1      # topology.py:1831-1833
+        width = int((input_width - self.kernel_size[1]) / self.stride[1]) + 1
+        depth = int((input_depth - self.kernel_size[2]) / self.stride[2]) + 1
+        self.conv_size = (height, width, depth)
+        self.conv_prod = int(np.prod(self.conv_size))
+        self.kernel_prod = int(np.prod(self.kernel_size))
+        if kwargs.get("w", None) is not None:
+            raise AttributeError(f"'{type(self).__name__}' object has no attribute 'out_channels' (the reference's w= shape "
+                                 "check, topology.py:1852-1857, reads an attribute it never sets)")
+        w = torch.rand(self.in_channels, self.n_filters * self.conv_prod, self.kernel_prod)
+        if (self.wmin != -np.inf).any() or (self.wmax != np.inf).any():
+            w = torch.clamp(w, self.wmin, self.wmax)
+        self.w = Parameter(w.contiguous(), requires_grad=False)
+        b = kwargs.get("b", None)
+        self.b = Parameter(torch.as_tensor(b, dtype=torch.float32) if b is not None else torch.empty(0), requires_grad=False)
+
+    def compute(self, s: torch.Tensor) -> torch.Tensor:
+        """topology.py:1866-1896 as the window kernel's receptive-field gather (``snn_b200_conn_compute``)."""
+        from . import _plan
+
+        return _plan.compute_single_connection(self, s)
+
+    def normalize(self) -> None:
+        """topology.py:1898-1909: every row of ``w`` viewed as ``[in_channels * n, kernel_prod]`` scaled to sum ``norm``
+        (a row that sums to zero becomes inf / NaN, as in the reference)."""
+        if self.norm is not None:
+            from . import _plan
+
+            _plan.normalize_single_connection(self)
+
+    def reset_state_variables(self) -> None:
+        """topology.py:1911-1917."""
+        super().reset_state_variables()
+        self.target.reset_state_variables()
+
+    def _check(self) -> None:
+        """The reference's errors at the first ``compute``, raised before anything runs.  ``int((in - k) / s) + 1``
+        truncates towards zero, so a kernel larger than the source can still give a conv size of 1 or more; unfold fails."""
+        C_, H, W, D = (int(v) for v in self.source.shape)
+        if any(k > n for k, n in zip(self.kernel_size, (H, W, D))) or min(self.kernel_size) < 1 or min(self.stride) < 1:
+            raise RuntimeError(f"LocalConnection3D: kernel_size {self.kernel_size} / stride {self.stride} do not fit a "
+                               f"{H} x {W} x {D} source (unfold fails)")
+        n = self.n_filters * self.conv_prod
+        if self.target.n != n:
+            raise RuntimeError(f"shape '[B, {', '.join(str(int(v)) for v in self.target.shape)}]' is invalid for the "
+                               f"LocalConnection3D output of {n} neurons per sample (n_filters * conv_prod)")
+        if tuple(self.w.shape) != (C_, n, self.kernel_prod):
+            raise RuntimeError(f"LocalConnection3D.w has shape {tuple(self.w.shape)}, expected {(C_, n, self.kernel_prod)}")
+
+    def _fill_desc(self, d: "_abi.SnnConn", dt: float, rule: bool = True) -> None:
+        self._check()
+        d.kind = _abi.SNN_CONN_LOCAL3D
+        if self.wmin.numel() != 1 or self.wmax.numel() != 1:
+            raise NotImplementedError("per-synapse wmin/wmax tensors are not supported by the CUDA core yet")
+        d.wmin = _scalar(self.wmin, "wmin")
+        d.wmax = _scalar(self.wmax, "wmax")
+        d.has_norm = int(self.norm is not None)
+        d.norm_abs = 0
+        d.norm = float(self.norm) if self.norm is not None else 0.0
+        d.dt_scale = 1.0
+        fill_local3d_geometry(d, self)
+        if rule:
+            self.update_rule._fill_desc(d)
+
+
+def fill_local3d_geometry(d: "_abi.SnnConn", conn) -> None:
+    """The SNN_CONN_LOCAL3D geometry of a LocalConnection3D (this package's or the reference's: the same attributes).  The
+    reference's axes H, W, D go to the depth, height and width fields, so that D stays the contiguous one."""
+    d.cin, d.din, d.hin, d.win = (int(v) for v in conn.source.shape)
+    d.cout, (d.dout, d.hout, d.wout) = int(conn.n_filters), (int(v) for v in conn.conv_size)
+    d.kd, d.kh, d.kw = (int(v) for v in conn.kernel_size)
+    d.sd, d.sh, d.sw = (int(v) for v in conn.stride)
+    d.pd = d.ph = d.pw = 0
+    d.dh = d.dw = 1
+
+
 def pool_out_shape(conn):
     """``[C, Hout, Wout]`` of a MaxPool2dConnection (this package's or the reference's: the same attributes), or the
     ``RuntimeError`` the reference's ``compute`` raises for its geometry.  ``F.max_pool2d`` without ceil mode; every window
@@ -1091,5 +1207,4 @@ def _unsupported(name: str, where: str):
 MaxPool1dConnection = _unsupported("MaxPool1dConnection", "topology.py:1028-1121")
 MaxPoo3dConnection = _unsupported("MaxPoo3dConnection", "topology.py:1214-1301")
 LocalConnection1D = _unsupported("LocalConnection1D", "topology.py:1487-1620")
-LocalConnection3D = _unsupported("LocalConnection3D", "topology.py:1770-1917")
 MeanFieldConnection = _unsupported("MeanFieldConnection", "topology.py:1920-2006")

@@ -9,7 +9,7 @@ a library that implements it — ``libsnn_b200.so`` on CUDA tensors, or the orac
 
 Covered: what ``bindsnet.models`` builds for the hot path — ``Input`` / ``LIFNodes`` / ``DiehlAndCookNodes`` layers,
 ``MulticompartmentConnection`` with one ``Weight`` feature (``MCC_learning.NoOp`` / ``PostPre``) and the classic
-``Connection`` and ``LocalConnection2D`` with ``learning.NoOp`` / ``PostPre`` / ``WeightDependentPostPre`` / ``Hebbian``,
+``Connection``, ``LocalConnection2D`` and ``LocalConnection3D`` with ``learning.NoOp`` / ``PostPre`` / ``WeightDependentPostPre`` / ``Hebbian``,
 ``Conv3dConnection`` with the updates the reference can run on it, ``Conv1dConnection`` with ``learning.NoOp`` /
 ``PostPre`` / ``WeightDependentPostPre`` / ``Hebbian``.  Every attribute is read where the
 reference keeps it (file:line in the comments); state tensors are handed over by pointer and updated in place.
@@ -186,6 +186,35 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
         if w.dtype != torch.float32 or not w.is_contiguous():
             raise TypeError("weights must be contiguous float32")
         d.w = w.data_ptr()
+        return
+    if type(conn).__name__ == "LocalConnection3D":
+        # topology.py:1770-1917: w [in_channels, n_filters * conv_prod, kernel_prod], b never read; the reference's axes
+        # H, W, D on the depth, height and width fields (include/snn_b200.h SNN_CONN_LOCAL3D), no padding, no dilation
+        from .network.topology import fill_local3d_geometry
+
+        if len(conn.source.shape) != 4:
+            raise NotImplementedError("LocalConnection3D from a source population other than [C, H, W, D]")
+        fill_local3d_geometry(d, conn)
+        d.kind = _abi.SNN_CONN_LOCAL3D
+        if (d.kd > d.din or d.kh > d.hin or d.kw > d.win) or int(conn.target.n) != d.cout * d.dout * d.hout * d.wout:
+            raise RuntimeError(f"LocalConnection3D: kernel_size {tuple(conn.kernel_size)} / stride {tuple(conn.stride)} on a "
+                               f"{list(conn.source.shape)} source do not give the target's {int(conn.target.n)} neurons")
+        d.has_norm = int(conn.norm is not None)                                           # topology.py:1898-1909
+        d.norm, d.norm_abs = (_f(conn.norm) if conn.norm is not None else 0.0), 0
+        rule = conn.update_rule
+        name = type(rule).__name__
+        d.rule = {"NoOp": _abi.SNN_RULE_NOOP, "PostPre": _abi.SNN_RULE_POSTPRE, "Hebbian": _abi.SNN_RULE_HEBBIAN,
+                  "WeightDependentPostPre": _abi.SNN_RULE_WDEP_POSTPRE}.get(name, -1)
+        if d.rule < 0:
+            raise NotImplementedError(f"learning rule {name} on a LocalConnection3D")
+        d.nu0, d.nu1 = _f(rule.nu[0]), _f(rule.nu[1])
+        d.reduction = _reduction_code(rule.reduction)
+        d.weight_decay = _f(rule.weight_decay)                                            # learning.py:85
+        d.wmin, d.wmax = _f(conn.wmin), _f(conn.wmax)
+        d.has_clamp = int((math.isfinite(d.wmin) or math.isfinite(d.wmax)) and name != "NoOp")   # learning.py:97-104
+        if conn.w.dtype != torch.float32 or not conn.w.is_contiguous():
+            raise TypeError("weights must be contiguous float32")
+        d.w = conn.w.data_ptr()
         return
     if type(conn).__name__ == "Conv3dConnection":
         # topology.py:847-1025: w [out, in, kd, kh, kw], b [out]; the geometry of F.conv3d (dilation 1: the constructor refuses

@@ -157,6 +157,27 @@ extern "C" {
                               decay and clamp.  normalize: each row of w viewed as [cout * cin, kw] scaled by
                               norm / (its sum, ascending), no guard against a zero sum.  No mask.  Generic tier only,
                               not with SNN_CONN_SPARSE or MCC features */
+#define SNN_CONN_LOCAL3D 8 /* LocalConnection3D: per-target (unshared) receptive-field weights, topology.py:1770-1917.
+                              The reference's source [cin, H, W, D] maps onto the conv fields with the innermost axis
+                              kept contiguous: H -> din / kd / sd / dout (the depth fields SNN_CONN_CONV3D overlays on the
+                              sparse storage), W -> hin / kh / sh / hout, D -> win / kw / sw / wout; so source neuron
+                              (ci, z, y, x) is ((ci * din + z) * hin + y) * win + x.  Each output size is
+                              (in - k) / s + 1 of a kernel that fits; pd = ph = pw = 0, dh = dw = 1; cout = n_filters.
+                              w is [cin, n, K] with K = kd * kh * kw, k = (kz * kh + ky) * kw + kx (the reference's
+                              flattening of its three unfolds); b is NULL.  Target n' = f * P + p, P = dout * hout * wout,
+                              p = (oz * hout + oy) * wout + ox, receives
+                                sum_ci ( sum_k s[ci, oz*sd + kz, oy*sh + ky, ox*sw + kx] * w[ci, n', k] )
+                              the inner sum over the spiking k ascending from +0, the outer one over ci ascending.
+                              Rules SNN_RULE_NONE / NOOP / POSTPRE / WDEP_POSTPRE / HEBBIAN, paired as on
+                              SNN_CONN_LOCAL2D: element (n', m), m < cin * K, is flat weight n' * cin * K + m, and its
+                              source neuron is the one at flat position (n' % P) * cin * K + m of the unfolded source in
+                              [cin, P, K] order (for cin = 1 the receptive field).
+                                U = reduce_b x_tgt[b, n'] * s_src[b, src],  V = reduce_b s_tgt[b, n'] * x_src[b, src]
+                              the samples in ascending b from +0, the terms of a silent spike skipped; then the rule,
+                              decay and clamp.  normalize: each row of w viewed as [cin * n, K] scaled by
+                              norm / (its sum, ascending k), no guard against a zero sum.  No mask.  Generic tier only,
+                              not with SNN_CONN_SPARSE, MCC features or per-neuron parameters; a library older than the
+                              kind refuses it with SNN_ERR_UNSUPPORTED */
 #define SNN_RULE_NONE 0        /* MCC_learning.NoOp: update() does nothing    MCC_learning.py:120-146 */
 #define SNN_RULE_NOOP 1        /* learning.NoOp: weight decay only, no clamp  learning.py:107-146     */
 #define SNN_RULE_POSTPRE 2     /* learning.PostPre._connection_update         learning.py:390-420     */

@@ -73,13 +73,13 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
     if ((o->delta_w || o->delta_theta) && (o->normalize || !net->learning || o->one_step)) return SNN_ERR_UNSUPPORTED;
     for (int c = 0; c < net->n_conns; ++c) {
         const snn_conn_t &C = net->conns[c];
-        const bool sparse = C.kind == SNN_CONN_SPARSE, pool = C.kind == SNN_CONN_MAXPOOL2D, local = C.kind == SNN_CONN_LOCAL2D;
+        const bool sparse = C.kind == SNN_CONN_SPARSE, pool = snn_is_maxpool(C.kind), local = C.kind == SNN_CONN_LOCAL2D;
         const bool conv3d = C.kind == SNN_CONN_CONV3D, conv1d = C.kind == SNN_CONN_CONV1D, local3d = C.kind == SNN_CONN_LOCAL3D;
         if (C.src < 0 || C.src >= net->n_layers || C.tgt < 0 || C.tgt >= net->n_layers) return SNN_ERR_BAD_ARG;
         if (pool ? (C.w || C.b) : (!C.w && !(sparse && C.nnz == 0))) return SNN_ERR_BAD_ARG;
         if (net->layers[C.tgt].kind == SNN_NODE_INPUT) return SNN_ERR_UNSUPPORTED;
         if (C.rule < SNN_RULE_NONE || C.rule > SNN_RULE_MSTDPET) return SNN_ERR_UNSUPPORTED;
-        if (C.kind < SNN_CONN_DENSE || C.kind > SNN_CONN_LOCAL3D) return SNN_ERR_UNSUPPORTED;
+        if (C.kind < SNN_CONN_DENSE || C.kind > SNN_CONN_MAXPOOL3D) return SNN_ERR_UNSUPPORTED;
         if (conv1d) {   // NoOp and the three unsupervised rules, no mask (snn_b200.h)
             const int rc = snn_conv1d_geometry_ok(C, net->layers[C.src].n, net->layers[C.tgt].n);
             if (rc != SNN_OK) return rc;
@@ -141,19 +141,17 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
         }
         // a PassThroughNodes layer carries 0 / 1 spikes: pooled ones in, none of a rule's traces (snn_b200.h)
         const bool pass_src = net->layers[C.src].kind == SNN_NODE_PASSTHROUGH, pass_tgt = net->layers[C.tgt].kind == SNN_NODE_PASSTHROUGH;
-        if (pass_tgt && !pool) return SNN_ERR_UNSUPPORTED;
+        if (pass_tgt && C.kind != SNN_CONN_MAXPOOL2D) return SNN_ERR_UNSUPPORTED;
         if ((pass_src || pass_tgt) && C.rule != SNN_RULE_NONE && C.rule != SNN_RULE_NOOP) return SNN_ERR_UNSUPPORTED;
     }
     return SNN_OK;
 }
 
-// the plan runs the pooling instantiation of the generic kernel: a MaxPool2dConnection, a LocalConnection2D, a
-// Conv3dConnection, a Conv1dConnection, a LocalConnection3D, or a layer of ann_to_snn's kinds
+// the plan runs the pooling instantiation of the generic kernel: a connection of a kind snn_pool_inst_kind names, or a
+// layer of ann_to_snn's kinds
 static bool has_pool(const snn_net_t *net) {
     for (int c = 0; c < net->n_conns; ++c)
-        if (net->conns[c].kind == SNN_CONN_MAXPOOL2D || net->conns[c].kind == SNN_CONN_LOCAL2D || net->conns[c].kind == SNN_CONN_CONV3D ||
-            net->conns[c].kind == SNN_CONN_CONV1D || net->conns[c].kind == SNN_CONN_LOCAL3D)
-            return true;
+        if (snn_pool_inst_kind(net->conns[c].kind)) return true;
     for (int l = 0; l < net->n_layers; ++l)
         if (net->layers[l].kind == SNN_NODE_SUBIF || net->layers[l].kind == SNN_NODE_PASSTHROUGH) return true;
     return false;
@@ -184,8 +182,7 @@ static bool has_syn(const snn_net_t *net) {
 static bool layer_needs_xpub(const snn_net_t *net, int l) {
     for (int c = 0; c < net->n_conns; ++c)
         if (net->conns[c].src == l && SNN_RULE_IS_STDP(net->conns[c].rule) && net->conns[c].kind != SNN_CONN_CONV2D &&
-            net->conns[c].kind != SNN_CONN_LOCAL2D && net->conns[c].kind != SNN_CONN_CONV3D && net->conns[c].kind != SNN_CONN_CONV1D &&
-            net->conns[c].kind != SNN_CONN_LOCAL3D)
+            !snn_pool_inst_kind(net->conns[c].kind))
             return true;
     return false;
 }
@@ -219,9 +216,7 @@ static size_t layout_generic(const snn_net_t *net, const snn_run_opts_t *o, char
         if (th) off += align_up(sizeof(int32_t) * 3 * L.n);
         bool wide_src = false;   // source of a dense connection with more than one gather block
         for (int c = 0; c < net->n_conns; ++c)
-            if (net->conns[c].src == l && net->conns[c].kind != SNN_CONN_CONV2D && net->conns[c].kind != SNN_CONN_MAXPOOL2D &&
-                net->conns[c].kind != SNN_CONN_LOCAL2D && net->conns[c].kind != SNN_CONN_CONV3D && net->conns[c].kind != SNN_CONN_CONV1D &&
-                net->conns[c].kind != SNN_CONN_LOCAL3D && nw > 32)
+            if (net->conns[c].src == l && net->conns[c].kind != SNN_CONN_CONV2D && !snn_pool_inst_kind(net->conns[c].kind) && nw > 32)
                 wide_src = true;
         if (N) N->layers[l].anyf = wide_src ? (uint32_t *)(ws + off) : nullptr;
         if (wide_src) off += align_up(sizeof(uint32_t) * 3 * B);
@@ -258,9 +253,9 @@ static size_t layout_generic(const snn_net_t *net, const snn_run_opts_t *o, char
         if (N) N->sp[c].out = (float *)(ws + off);
         off += align_up(sizeof(float) * B * nt);
     }
-    // MaxPool2dConnections: the second slot of the rates (pool_rate_slot)
+    // MaxPool2d / MaxPoo3dConnections: the second slot of the rates (pool_rate_slot)
     for (int c = 0; c < net->n_conns; ++c) {
-        if (net->conns[c].kind != SNN_CONN_MAXPOOL2D) continue;
+        if (!snn_is_maxpool(net->conns[c].kind)) continue;
         if (N) N->pool_r1[c] = (float *)(ws + off);
         off += align_up(sizeof(float) * B * (size_t)net->layers[net->conns[c].src].n);
     }
@@ -280,11 +275,9 @@ int snn_b200_last_launch_count(void) { return g_last_launches; }
 // (net: the plan strip_pn left; pn: some layer carries per-neuron parameters)
 static int select_tier(const snn_net_t *net, const snn_run_opts_t *opts, bool pn) {
     if (validate(net, opts) != SNN_OK) return 0;
-    // one extra instantiation of the generic kernel each for sparse, feature and pooling plans (pooling: also plans with
-    // a LocalConnection2D, a LocalConnection3D, a Conv3dConnection, a Conv1dConnection, SubtractiveResetIFNodes or
-    // PassThroughNodes), not
-    // combinations
-    // (and one for plans with per-synapse bounds or rates)
+    // one extra instantiation of the generic kernel each for sparse, feature and pooling plans (pooling: every kind
+    // snn_pool_inst_kind names, and SubtractiveResetIFNodes or PassThroughNodes), not combinations (and one for plans
+    // with per-synapse bounds or rates)
     if ((int)has_sparse(net) + (int)has_feat(net) + (int)has_pool(net) + (int)has_syn(net) > 1) return 0;
     // per-neuron parameters: two more instantiations, alone or with per-synapse tensors; the fused kernels read scalars
     if (pn) {

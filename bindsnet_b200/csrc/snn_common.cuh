@@ -97,35 +97,47 @@ struct DevNet {
     int32_t sp_units;             // sparse gather units of a step (0: the plan has no SparseConnection)
     DevSparse sp[SNN_MAX_CONNS];
     int32_t any_feat;             // some MCC connection carries Probability / Mask / Intensity features
-    int32_t any_pool;             // some connection is a MaxPool2dConnection (SNN_CONN_MAXPOOL2D), a LocalConnection2D
-                                  // (SNN_CONN_LOCAL2D), a Conv3dConnection (SNN_CONN_CONV3D), a Conv1dConnection
-                                  // (SNN_CONN_CONV1D) or a LocalConnection3D (SNN_CONN_LOCAL3D), or some layer is an SNN_NODE_SUBIF / SNN_NODE_PASSTHROUGH one: the
-                                  // plan runs the POOL instantiation
-    float *pool_r1[SNN_MAX_CONNS];   // MaxPool2dConnection: the workspace slot of its rates (pool_rate_slot)
+    int32_t any_pool;             // some connection is of a kind snn_pool_inst_kind names, or some layer is an
+                                  // SNN_NODE_SUBIF / SNN_NODE_PASSTHROUGH one: the plan runs the POOL instantiation
+    float *pool_r1[SNN_MAX_CONNS];   // MaxPool2d / MaxPoo3dConnection: the workspace slot of its rates (pool_rate_slot)
 };
 
-// A MaxPool2dConnection's rates, double-buffered: the gather of step t reads slot pool_rate_slot(T, t), where slot 0 is
-// the caller's snn_conn_t::pool_rates and slot 1 DevNet::pool_r1, so that the last step's rates are the caller's.  The
-// rates step t reads are written one slot earlier, by whoever finalises the spikes they fold in (pool_rate_step).
-// A MaxPool2dConnection's geometry (snn_b200.h): cin = cout, the layer sizes, F.max_pool2d's output size (no ceil mode) and
-// padding limit (at most half the kernel), and at least one element inside the image in every window.
+// A MaxPool2dConnection's or MaxPoo3dConnection's rates, double-buffered: the gather of step t reads slot
+// pool_rate_slot(T, t), where slot 0 is the caller's snn_conn_t::pool_rates and slot 1 DevNet::pool_r1, so that the last
+// step's rates are the caller's.  The rates step t reads are written one slot earlier, by whoever finalises the spikes
+// they fold in (pool_rate_step).
+__host__ __device__ __forceinline__ bool snn_is_maxpool(int kind) { return kind == SNN_CONN_MAXPOOL2D || kind == SNN_CONN_MAXPOOL3D; }
+// The connection kinds that only the POOL instantiation of the generic kernel runs (the plan selects it when one is
+// present); none of them is gathered through the dense path of phase 1.
+__host__ __device__ __forceinline__ bool snn_pool_inst_kind(int kind) {
+    return snn_is_maxpool(kind) || kind == SNN_CONN_LOCAL2D || kind == SNN_CONN_CONV3D || kind == SNN_CONN_CONV1D ||
+           kind == SNN_CONN_LOCAL3D;
+}
+// One axis of a pooling geometry: F.max_pool2d / F.max_pool3d's output size (no ceil mode) and padding limit (at most
+// half the kernel), and at least one element inside the input in every window.
+static inline bool snn_pool_axis_ok(int in, int out, int k, int s, int p, int d) {
+    if (in < 1 || k < 1 || s < 1 || d < 1 || p < 0 || p > k / 2) return false;
+    const int e = in + 2 * p - d * (k - 1) - 1;
+    if (e < 0 || out != e / s + 1) return false;
+    for (int o = 0; o < out; ++o) {
+        bool any = false;
+        for (int j = 0; j < k && !any; ++j) any = o * s - p + j * d >= 0 && o * s - p + j * d < in;
+        if (!any) return false;
+    }
+    return true;
+}
+// A MaxPool2dConnection's or MaxPoo3dConnection's geometry (snn_b200.h): cin = cout, the layer sizes and every axis
+// (snn_pool_axis_ok); the depth fields are read for SNN_CONN_MAXPOOL3D only (on SNN_CONN_MAXPOOL2D they overlay the NULL
+// sparse pointers).
 static inline int snn_pool_geometry_ok(const snn_conn_t &C, int n_src, int n_tgt) {
     if (!C.pool_rates) return SNN_ERR_BAD_ARG;
-    if (C.cin != C.cout || C.cin < 1 || (long long)C.cin * C.hin * C.win != n_src || (long long)C.cout * C.hout * C.wout != n_tgt) return SNN_ERR_BAD_ARG;
-    if (C.kh < 1 || C.kw < 1 || C.sh < 1 || C.sw < 1 || C.dh < 1 || C.dw < 1 || C.ph < 0 || C.pw < 0) return SNN_ERR_BAD_ARG;
-    if (C.ph > C.kh / 2 || C.pw > C.kw / 2) return SNN_ERR_BAD_ARG;
-    const int eh = C.hin + 2 * C.ph - C.dh * (C.kh - 1) - 1, ew = C.win + 2 * C.pw - C.dw * (C.kw - 1) - 1;
-    if (eh < 0 || ew < 0 || C.hout != eh / C.sh + 1 || C.wout != ew / C.sw + 1) return SNN_ERR_BAD_ARG;
-    for (int o = 0; o < C.hout; ++o) {
-        bool any = false;
-        for (int k = 0; k < C.kh && !any; ++k) any = o * C.sh - C.ph + k * C.dh >= 0 && o * C.sh - C.ph + k * C.dh < C.hin;
-        if (!any) return SNN_ERR_BAD_ARG;
-    }
-    for (int o = 0; o < C.wout; ++o) {
-        bool any = false;
-        for (int k = 0; k < C.kw && !any; ++k) any = o * C.sw - C.pw + k * C.dw >= 0 && o * C.sw - C.pw + k * C.dw < C.win;
-        if (!any) return SNN_ERR_BAD_ARG;
-    }
+    const bool d3 = C.kind == SNN_CONN_MAXPOOL3D;
+    const long long din = d3 ? C.din : 1, dout = d3 ? C.dout : 1;
+    if (C.cin != C.cout || C.cin < 1 || (long long)C.cin * din * C.hin * C.win != n_src || (long long)C.cout * dout * C.hout * C.wout != n_tgt)
+        return SNN_ERR_BAD_ARG;
+    if (d3 && !snn_pool_axis_ok(C.din, C.dout, C.kd, C.sd, C.pd, C.dd)) return SNN_ERR_BAD_ARG;
+    if (!snn_pool_axis_ok(C.hin, C.hout, C.kh, C.sh, C.ph, C.dh) || !snn_pool_axis_ok(C.win, C.wout, C.kw, C.sw, C.pw, C.dw))
+        return SNN_ERR_BAD_ARG;
     return SNN_OK;
 }
 
@@ -207,7 +219,7 @@ static inline int snn_syn_check(const snn_conn_t &C) {
 
 __host__ __device__ __forceinline__ int pool_rate_slot(int T, int t) { return (T - 1 - t) & 1; }
 __device__ __forceinline__ float *pool_rates_at(const DevNet &N, int c, int slot) { return slot ? N.pool_r1[c] : N.conns[c].pool_rates; }
-// MaxPool2dConnection.compute step 1 (topology.py:1175-1176): r -= decay * r; r += s
+// MaxPool2dConnection / MaxPoo3dConnection.compute step 1 (topology.py:1175-1176, :1265-1266): r -= decay * r; r += s
 __host__ __device__ __forceinline__ float pool_rate_update(float r, float decay, bool s) {
     r = r - decay * r;
     return r + (s ? 1.0f : 0.0f);

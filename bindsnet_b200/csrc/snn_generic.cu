@@ -53,8 +53,8 @@ __device__ __forceinline__ void sparse_unit(const DevNet &N, int u, int &c, int 
 // code (and register allocation) is exactly what it is without the feature.
 // FEAT: the plan holds a MulticompartmentConnection with Probability / Mask / Intensity features (snn_b200.h); only the
 // dense gather of phase 1 differs.  The two are not combined in one plan.
-// POOL: the plan holds a MaxPool2dConnection, a LocalConnection2D, a LocalConnection3D, a Conv3dConnection, a
-// Conv1dConnection or a layer of ann_to_snn's kinds (SNN_NODE_SUBIF, SNN_NODE_PASSTHROUGH, whose s is float32): phase 1
+// POOL: the plan holds a connection of a kind snn_pool_inst_kind names (MaxPool2dConnection, MaxPoo3dConnection,
+// LocalConnection2D, LocalConnection3D, Conv3dConnection, Conv1dConnection) or a layer of ann_to_snn's kinds (SNN_NODE_SUBIF, SNN_NODE_PASSTHROUGH, whose s is float32): phase 1
 // gathers the pooled spikes, the 2-D and 3-D local receptive fields and the 3-D and 1-D convolutions and steps those
 // layers, the learning phase runs the local and Conv1d rules and the Conv3d decay over the grid, normalize() scales the local rows and the 3-D and 1-D filters, and every
 // finalised spike of a pooling source advances its rates (pool_rate_step); the prologue writes the rates of step 0.  Not
@@ -112,11 +112,12 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                     for (size_t k = start; k < ne; k += stride) Ms.el[1][k] = Ms.el[0][k];
                 }
             }
-        // MaxPool2dConnection rates of step 0: the caller's rates advanced by the incoming spikes s(-1); in one-step mode
-        // with the source earlier in the insertion order step 0 advances them itself, from slot pool_rate_slot(T, -1)
+        // MaxPool2d / MaxPoo3dConnection rates of step 0: the caller's rates advanced by the incoming spikes s(-1); in
+        // one-step mode with the source earlier in the insertion order step 0 advances them itself, from slot
+        // pool_rate_slot(T, -1)
         for (int c = 0; POOL && N.T > 0 && c < N.n_conns; ++c) {
             const snn_conn_t &C = N.conns[c];
-            if (C.kind != SNN_CONN_MAXPOOL2D || C.src != li || j >= D.L.n) continue;
+            if (!snn_is_maxpool(C.kind) || C.src != li || j >= D.L.n) continue;
             const bool cur = N.one_step && C.src < C.tgt;
             float *dst = pool_rates_at(N, c, pool_rate_slot(N.T, cur ? -1 : 0));
             for (int b = warp; b < N.B; b += SNN_GEN_WARPS) {
@@ -285,9 +286,8 @@ static int plan_units(DevNet &N, int cap) {
         const snn_conn_t &C = N.conns[c];
         N.p3_first[c] = p3;
         N.p3_rc[c] = 0;
-        if (!N.learning || C.rule == SNN_RULE_NONE || C.kind == SNN_CONN_CONV2D || C.kind == SNN_CONN_SPARSE || C.kind == SNN_CONN_MAXPOOL2D ||
-            C.kind == SNN_CONN_LOCAL2D || C.kind == SNN_CONN_CONV3D || C.kind == SNN_CONN_CONV1D || C.kind == SNN_CONN_LOCAL3D)
-            continue;   // (a MaxPool2dConnection has no weights to update; conv and local rules are spread over the grid)
+        if (!N.learning || C.rule == SNN_RULE_NONE || C.kind == SNN_CONN_CONV2D || C.kind == SNN_CONN_SPARSE || snn_pool_inst_kind(C.kind))
+            continue;   // (a pooling connection has no weights to update; conv and local rules are spread over the grid)
         const int nwS = N.layers[C.src].nw, nwT = N.layers[C.tgt].nw;
         if (SNN_RULE_IS_MSTDP(C.rule)) { N.p3_rc[c] = 1; p3 += nwS; continue; }
         int rc = ceil_div(cap, nwT);
@@ -311,8 +311,7 @@ static int plan_units(DevNet &N, int cap) {
     if (spu > units) units = spu;
     bool conv_rule = false;
     for (int c = 0; c < N.n_conns; ++c)
-        if (N.learning && (N.conns[c].kind == SNN_CONN_CONV2D || N.conns[c].kind == SNN_CONN_LOCAL2D || N.conns[c].kind == SNN_CONN_CONV3D ||
-                           N.conns[c].kind == SNN_CONN_CONV1D || N.conns[c].kind == SNN_CONN_LOCAL3D) &&
+        if (N.learning && (N.conns[c].kind == SNN_CONN_CONV2D || snn_pool_inst_kind(N.conns[c].kind)) && !snn_is_maxpool(N.conns[c].kind) &&
             N.conns[c].rule != SNN_RULE_NONE)
             conv_rule = true;
     int grid = conv_rule ? cap : (int)(units < cap ? units : cap);

@@ -115,20 +115,22 @@ __global__ void __launch_bounds__(256) conv_compute_kernel(snn_conn_t C, int ns,
     }
 }
 
-// MaxPool2dConnection.compute (topology.py:1163-1185), step 1: the rates advance by the spikes, in place.
+// MaxPool2dConnection / MaxPoo3dConnection.compute (topology.py:1163-1185, :1255-1277), step 1: the rates advance by
+// the spikes, in place.
 __global__ void __launch_bounds__(256) pool_rates_kernel(snn_conn_t C, size_t total, const uint8_t *__restrict__ s) {
     for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < total; k += (size_t)gridDim.x * blockDim.x)
         C.pool_rates[k] = pool_rate_update(C.pool_rates[k], C.pool_decay, s[k] != 0);
 }
 
-// Steps 2-3: the spike at the window's first maximum of the updated rates (the window gather's pool_argmax); thread = one
-// target neuron of one sample.
+// Steps 2-3: the spike at the window's first maximum of the updated rates (the window gather's pool_argmax; D3: the
+// 3-D window); thread = one target neuron of one sample.
+template <bool D3>
 __global__ void __launch_bounds__(256) pool_compute_kernel(snn_conn_t C, int ns, int nt, int B, const uint8_t *__restrict__ s,
                                                            float *__restrict__ out) {
     const size_t total = (size_t)B * nt;
     for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < total; k += (size_t)gridDim.x * blockDim.x) {
         const int b = (int)(k / nt), j = (int)(k - (size_t)b * nt);
-        out[k] = s[(size_t)b * ns + pool_argmax(C, C.pool_rates + (size_t)b * ns, j)] ? 1.0f : 0.0f;
+        out[k] = s[(size_t)b * ns + pool_argmax<D3>(C, C.pool_rates + (size_t)b * ns, j)] ? 1.0f : 0.0f;
     }
 }
 
@@ -330,19 +332,20 @@ extern "C" {
 
 int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, int32_t B, const uint8_t *s, float *out,
                           void *stream) {
-    if (!conn || (!conn->w && !(conn->kind == SNN_CONN_SPARSE && conn->nnz == 0) && conn->kind != SNN_CONN_MAXPOOL2D) || !s || !out ||
+    if (!conn || (!conn->w && !(conn->kind == SNN_CONN_SPARSE && conn->nnz == 0) && !snn_is_maxpool(conn->kind)) || !s || !out ||
         n_src <= 0 || n_tgt <= 0 || B <= 0)
         return SNN_ERR_BAD_ARG;
     // (on SNN_CONN_DENSE this storage holds the per-synapse tensors, which the gather does not read)
     const bool feat = conn->kind == SNN_CONN_MCC && (conn->f_prob || conn->f_mask || conn->f_int);
     if (conn->kind != SNN_CONN_MCC && conn->kind != SNN_CONN_DENSE && (conn->f_prob || conn->f_mask || conn->f_int)) return SNN_ERR_BAD_ARG;
-    if (conn->kind == SNN_CONN_MAXPOOL2D) {   // updates conn->pool_rates [B, n_src] in place, then writes [B, n_tgt]
+    if (snn_is_maxpool(conn->kind)) {   // updates conn->pool_rates [B, n_src] in place, then writes [B, n_tgt]
         const int rc = snn_pool_geometry_ok(*conn, n_src, n_tgt);
         if (rc != SNN_OK || conn->b) return rc != SNN_OK ? rc : SNN_ERR_BAD_ARG;
         const size_t total = (size_t)B * n_src, tout = (size_t)B * n_tgt;
         SNN_LAUNCH(pool_rates_kernel, (int)((total + 255) / 256 < 4736 ? (total + 255) / 256 : 4736), 256, 0, (cudaStream_t)stream, *conn, total, s);
-        SNN_LAUNCH(pool_compute_kernel, (int)((tout + 255) / 256 < 4736 ? (tout + 255) / 256 : 4736), 256, 0, (cudaStream_t)stream, *conn, n_src, n_tgt,
-                   B, s, out);
+        const int blocks = (int)((tout + 255) / 256 < 4736 ? (tout + 255) / 256 : 4736);
+        if (conn->kind == SNN_CONN_MAXPOOL3D) SNN_LAUNCH(pool_compute_kernel<true>, blocks, 256, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
+        else SNN_LAUNCH(pool_compute_kernel<false>, blocks, 256, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
         return cuda_rc(cudaGetLastError());
     }
     if (conn->kind == SNN_CONN_LOCAL2D) {

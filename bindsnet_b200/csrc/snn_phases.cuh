@@ -479,7 +479,8 @@ __device__ __forceinline__ float gather_local2d(const snn_conn_t &C, const uint3
 }
 
 // ---------------------------------------------------------------------------------------
-// MaxPool2dConnection (SNN_CONN_MAXPOOL2D, topology.py:1124-1211).
+// MaxPool2dConnection (SNN_CONN_MAXPOOL2D, topology.py:1124-1211) and MaxPoo3dConnection (SNN_CONN_MAXPOOL3D,
+// :1214-1301).
 //
 // The rates the gather of step t reads fold in the spikes that gather reads: step t - 1's (slot rd), or step t's in
 // one-step mode when the source comes earlier in the insertion order (`cur`).  Whoever finalises source neuron k of a
@@ -489,7 +490,7 @@ __device__ __forceinline__ float gather_local2d(const snn_conn_t &C, const uint3
 __device__ __forceinline__ void pool_rate_step(const DevNet &N, int li, size_t k, int t, bool sf) {
     for (int c = 0; c < N.n_conns; ++c) {
         const snn_conn_t &C = N.conns[c];
-        if (C.kind != SNN_CONN_MAXPOOL2D || C.src != li) continue;
+        if (!snn_is_maxpool(C.kind) || C.src != li) continue;
         const bool cur = N.one_step && C.src < C.tgt;
         const int tw = cur ? t : t + 1;   // the step whose gather reads what is written here
         if (tw >= N.T) continue;
@@ -498,32 +499,41 @@ __device__ __forceinline__ void pool_rate_step(const DevNet &N, int li, size_t k
     }
 }
 
-// The source neuron whose spike target neuron j = (ch, oy, ox) of a sample receives: the first maximum of the rates `r`
-// ([C, hin, win] of that sample) over the window — row-major window order, padding never chosen, strict comparison (an
-// equal rate, -0 against +0 included, keeps the earlier element), a NaN taking over as it does in F.max_pool2d's CPU
-// kernel.  Plan validation (snn_pool_geometry_ok) guarantees a valid element in every window.
+// The source neuron whose spike target neuron j = (ch, oy, ox) of a sample receives (D3: j = (ch, oz, oy, ox)): the first
+// maximum of the rates `r` ([C, hin, win] of that sample; D3: [C, din, hin, win]) over the window — row-major window
+// order ((kz,) ky, kx), padding never chosen, strict comparison (an equal rate, -0 against +0 included, keeps the earlier
+// element), a NaN taking over as it does in F.max_pool2d's / F.max_pool3d's CPU kernel.  Only D3 reads the depth fields
+// (on a MaxPool2dConnection they overlay the NULL sparse pointers).  Plan validation (snn_pool_geometry_ok) guarantees a
+// valid element in every window.
+template <bool D3 = false>
 __device__ __forceinline__ int pool_argmax(const snn_conn_t &C, const float *r, int j) {
-    const int L = C.hout * C.wout, ch = j / L, l = j - ch * L, oy = l / C.wout, ox = l - oy * C.wout;
-    const int HW = C.hin * C.win;
-    const float *rc = r + (size_t)ch * HW;
+    const int L = C.hout * C.wout * (D3 ? C.dout : 1), ch = j / L, l = j - ch * L;
+    const int oz = D3 ? l / (C.hout * C.wout) : 0, lp = D3 ? l - oz * (C.hout * C.wout) : l, oy = lp / C.wout, ox = lp - oy * C.wout;
+    const int HW = C.hin * C.win, V = HW * (D3 ? C.din : 1);
+    const float *rc = r + (size_t)ch * V;
     float best = 0.0f;
     int idx = 0;
     bool any = false;
-    for (int ky = 0; ky < C.kh; ++ky) {
-        const int iy = oy * C.sh - C.ph + ky * C.dh;
-        if (iy < 0 || iy >= C.hin) continue;
-        for (int kx = 0; kx < C.kw; ++kx) {
-            const int ix = ox * C.sw - C.pw + kx * C.dw;
-            if (ix < 0 || ix >= C.win) continue;
-            const float v = __ldcg(rc + iy * C.win + ix);
-            if (!any || v > best || v != v) { best = v; idx = iy * C.win + ix; any = true; }
+    const int kd = D3 ? C.kd : 1;
+    for (int kz = 0; kz < kd; ++kz) {
+        const int iz = D3 ? oz * C.sd - C.pd + kz * C.dd : 0;
+        if (D3 && (iz < 0 || iz >= C.din)) continue;
+        for (int ky = 0; ky < C.kh; ++ky) {
+            const int iy = oy * C.sh - C.ph + ky * C.dh;
+            if (iy < 0 || iy >= C.hin) continue;
+            for (int kx = 0; kx < C.kw; ++kx) {
+                const int ix = ox * C.sw - C.pw + kx * C.dw;
+                if (ix < 0 || ix >= C.win) continue;
+                const float v = __ldcg(rc + (D3 ? iz * HW : 0) + iy * C.win + ix);
+                if (!any || v > best || v != v) { best = v; idx = (D3 ? iz * HW : 0) + iy * C.win + ix; any = true; }
+            }
         }
     }
-    return ch * HW + idx;
+    return ch * V + idx;
 }
 
 // Final spikes of one neuron of one sample: traces (nodes.py:96-103), clamp / unclamp (network.py:415-429),
-// recordings, and (POOL) the next rate of every MaxPool2dConnection leaving the layer.  Returns the spike that is published.
+// recordings, and (POOL) the next rate of every MaxPool2d / MaxPoo3dConnection leaving the layer.  Returns the spike that is published.
 // (POOL) A PassThroughNodes layer has no traces (its forward never reaches Nodes.forward) and a float32 s.
 // (PN) `P` holds the neuron's trace decay and scale (snn_b200.h SNN_NODE_PN).
 template <bool POOL, bool PN = false>
@@ -687,9 +697,7 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
         for (int q = 0; q < 4; ++q) {
             fwn[q] = 0u; afn[q] = 1u;
             if (q < ncl && b < b1 && N.conns[cl[q]].kind != SNN_CONN_CONV2D && !(SPARSE && N.conns[cl[q]].kind == SNN_CONN_SPARSE) &&
-                !(POOL && (N.conns[cl[q]].kind == SNN_CONN_MAXPOOL2D || N.conns[cl[q]].kind == SNN_CONN_LOCAL2D ||
-                           N.conns[cl[q]].kind == SNN_CONN_CONV3D || N.conns[cl[q]].kind == SNN_CONN_CONV1D ||
-                           N.conns[cl[q]].kind == SNN_CONN_LOCAL3D))) {
+                !(POOL && snn_pool_inst_kind(N.conns[cl[q]].kind))) {
                 const snn_conn_t &C = N.conns[cl[q]];
                 const DevLayer &S = N.layers[C.src];
                 const int slot = (N.one_step && C.src < li) ? wr : rd;
@@ -741,10 +749,10 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
                 } else {
                     p = gather_conv<false, false>(C, gsb, nullptr, 0, j, valid, c == conv_c ? geo : conv_geo(C, j, valid));
                 }
-            } else if (POOL && C.kind == SNN_CONN_MAXPOOL2D) {   // rates of this step: pool_rate_step / the prologue
+            } else if (POOL && snn_is_maxpool(C.kind)) {   // rates of this step: pool_rate_step / the prologue
                 const float *r = pool_rates_at(N, c, pool_rate_slot(N.T, t)) + (size_t)b * S.L.n;
                 const uint32_t *sb = S.bits + ((size_t)slot * B + b) * S.nw;
-                const int i = valid ? pool_argmax(C, r, j) : 0;
+                const int i = !valid ? 0 : C.kind == SNN_CONN_MAXPOOL3D ? pool_argmax<true>(C, r, j) : pool_argmax<false>(C, r, j);
                 p = (valid && ((__ldcg(sb + (i >> 5)) >> (i & 31)) & 1u)) ? 1.0f : 0.0f;
             } else if (POOL && C.kind == SNN_CONN_CONV3D) {
                 const uint32_t *gsb = S.bits + ((size_t)slot * B + b) * S.nw;

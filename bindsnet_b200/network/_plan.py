@@ -6,12 +6,13 @@ single-operator entry points.  Everything here is host bookkeeping — no arithm
 """
 from __future__ import annotations
 
+import math
 from typing import Dict, List, Optional, Tuple
 
 import torch
 
 from .. import _abi, _backend
-from .topology import LocalConnection2D, MaxPool2dConnection
+from .topology import LocalConnection2D, _MaxPoolConnection
 
 
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
@@ -94,7 +95,7 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
         rule0 = conn._weight().learning_rule   # MulticompartmentConnection.update never reaches it with manual_update
     if rule and hasattr(rule0, "_prepare"):  # rules with state of their own (MSTDP): allocate for this batch size / device
         rule0._prepare(B, conn.w.device, rule_kwargs or {})
-    if isinstance(conn, MaxPool2dConnection):   # no weights: the rates buffer and the geometry are all there is
+    if isinstance(conn, _MaxPoolConnection):   # no weights: the rates buffer and the geometry are all there is
         conn._check((B, *conn.source.shape))
         conn._fill_desc(d, dt, rule)
         return
@@ -304,7 +305,7 @@ def build_net(
     masks = getattr(network, "_conn_masks", None) or {}
     by_id = {id(layer): i for i, layer in enumerate(network.layers.values())}
     for i, ((src, tgt), conn) in enumerate(network.connections.items()):
-        if network.learning and isinstance(conn, MaxPool2dConnection):
+        if network.learning and isinstance(conn, _MaxPoolConnection):
             raise AttributeError(conn._no_w_message())   # the reference fails in the first step's update
         # the source is the connection's own source layer (network.py:226-248 reads connection.source.s): ann_to_snn's
         # keys name the previous ANN child, which need not be a layer
@@ -319,11 +320,10 @@ def build_net(
         check_passthrough(net, i, type(conn).__name__)
     conns = [net.conns[i] for i in range(net.n_conns)]
     layers = [net.layers[i] for i in range(net.n_layers)]
-    pool_kinds = (_abi.SNN_CONN_MAXPOOL2D, _abi.SNN_CONN_LOCAL2D, _abi.SNN_CONN_CONV3D, _abi.SNN_CONN_CONV1D, _abi.SNN_CONN_LOCAL3D)
-    if (any(d.kind in pool_kinds for d in conns) or any(d.kind in CONVERSION_KINDS for d in layers)) and any(
+    if (any(d.kind in POOL_INST_KINDS for d in conns) or any(d.kind in CONVERSION_KINDS for d in layers)) and any(
             d.kind == _abi.SNN_CONN_SPARSE or d.f_prob or d.f_mask or d.f_int for d in conns):
-        raise NotImplementedError("a network with a MaxPool2dConnection, LocalConnection2D, Conv3dConnection, Conv1dConnection, "
-                                  "LocalConnection3D, SubtractiveResetIFNodes or PassThroughNodes and a SparseConnection or MulticompartmentConnection "
+        raise NotImplementedError("a network with a MaxPool2dConnection, MaxPoo3dConnection, LocalConnection2D, Conv3dConnection, "
+                                  "Conv1dConnection, LocalConnection3D, SubtractiveResetIFNodes or PassThroughNodes and a SparseConnection or MulticompartmentConnection "
                                   "features is not implemented by the CUDA core (each has its own instantiation of the window kernel)")
     check_neuron_params(layers, conns)
     return net, keep
@@ -335,16 +335,18 @@ def check_neuron_params(layers, conns) -> None:
     or pooling one."""
     if not any(d.kind & _abi.SNN_NODE_PN for d in layers):
         return
-    pool_kinds = (_abi.SNN_CONN_MAXPOOL2D, _abi.SNN_CONN_LOCAL2D, _abi.SNN_CONN_CONV3D, _abi.SNN_CONN_CONV1D, _abi.SNN_CONN_LOCAL3D)
-    if any(d.kind == _abi.SNN_CONN_SPARSE or d.kind in pool_kinds or (d.kind == _abi.SNN_CONN_MCC and (d.f_prob or d.f_mask or d.f_int))
+    if any(d.kind == _abi.SNN_CONN_SPARSE or d.kind in POOL_INST_KINDS or (d.kind == _abi.SNN_CONN_MCC and (d.f_prob or d.f_mask or d.f_int))
            for d in conns) or any(d.kind in CONVERSION_KINDS for d in layers):
         raise NotImplementedError("per-neuron parameter tensors in a network with a SparseConnection, MulticompartmentConnection "
-                                  "features, a MaxPool2dConnection, LocalConnection2D, Conv3dConnection, Conv1dConnection, "
-                                  "LocalConnection3D, SubtractiveResetIFNodes or PassThroughNodes are not implemented by the CUDA core (each has its own instantiation of "
+                                  "features, a MaxPool2dConnection, MaxPoo3dConnection, LocalConnection2D, Conv3dConnection, "
+                                  "Conv1dConnection, LocalConnection3D, SubtractiveResetIFNodes or PassThroughNodes are not implemented by the CUDA core (each has its own instantiation of "
                                   "the window kernel)")
 
 
 CONVERSION_KINDS = (_abi.SNN_NODE_SUBIF, _abi.SNN_NODE_PASSTHROUGH)
+# the connection kinds that only the pooling instantiation of the window kernel runs (snn_common.cuh snn_pool_inst_kind)
+POOL_INST_KINDS = (_abi.SNN_CONN_MAXPOOL2D, _abi.SNN_CONN_MAXPOOL3D, _abi.SNN_CONN_LOCAL2D, _abi.SNN_CONN_CONV3D, _abi.SNN_CONN_CONV1D,
+                   _abi.SNN_CONN_LOCAL3D)
 
 
 def check_passthrough(net: "_abi.SnnNet", i: int, what: str) -> None:
@@ -373,7 +375,7 @@ def compute_single_connection(conn, s: torch.Tensor, draw: Optional[Tuple[int, i
     """``conn.compute(s)``: ``[B, *target.shape]`` currents for spikes ``s``.  ``draw`` = (seed, step, connection index)
     of a Probability feature's draw; by default a fresh seed from torch's CPU generator, step 0, index 0."""
     B = s.shape[0]
-    if isinstance(conn, MaxPool2dConnection):
+    if isinstance(conn, _MaxPoolConnection):
         return _compute_pool(conn, s)
     _backend.require_cuda(conn.w, "connection weights")
     su8 = _as_u8(s if s.dtype in (torch.bool, torch.uint8) else (s != 0)).reshape(B, -1).contiguous()
@@ -389,7 +391,8 @@ def compute_single_connection(conn, s: torch.Tensor, draw: Optional[Tuple[int, i
 
 
 def _compute_pool(conn, s: torch.Tensor) -> torch.Tensor:
-    """``MaxPool2dConnection.compute(s)``: the rates advance in place, ``[B, C, Hout, Wout]`` pooled spikes."""
+    """``MaxPool2dConnection.compute(s)`` / ``MaxPoo3dConnection.compute(s)``: the rates advance in place, ``[B, C,
+    Hout, Wout]`` / ``[B, C, Dout, Hout, Wout]`` pooled spikes."""
     fr = conn.firing_rates
     _backend.require_cuda(fr, "firing_rates")
     conn._check(tuple(s.shape))
@@ -397,8 +400,8 @@ def _compute_pool(conn, s: torch.Tensor) -> torch.Tensor:
     su8 = _as_u8(s if s.dtype in (torch.bool, torch.uint8) else (s != 0)).reshape(B, -1).contiguous().to(fr.device)
     d = _abi.SnnConn()
     conn._fill_desc(d, 1.0)
-    shape = (d.cout, d.hout, d.wout)
-    out = torch.empty(B, d.cout * d.hout * d.wout, dtype=torch.float32, device=fr.device)
+    shape = conn._out_shape()
+    out = torch.empty(B, math.prod(shape), dtype=torch.float32, device=fr.device)
     _backend.conn_compute(d, conn.source.n, out.shape[1], B, su8, out)
     return out.view(B, *shape)
 

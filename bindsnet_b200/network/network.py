@@ -209,7 +209,7 @@ class Network(torch.nn.Module):
     def _stage_conn_masks(self, masks, dev: torch.device):
         """``masks={(source, target): bool tensor}`` (network.py:279-280,321): weights to clamp to zero after every
         step's update (AbstractConnection.update, topology.py:127-131)."""
-        from .topology import Connection, MaxPool2dConnection, SparseConnection
+        from .topology import Connection, SparseConnection, _MaxPoolConnection
 
         out = {}
         for key, m in (masks or {}).items():
@@ -220,7 +220,7 @@ class Network(torch.nn.Module):
             conn = self.connections[key]
             if isinstance(conn, SparseConnection):
                 raise NotImplementedError("Mask isn't supported for SparseConnection")   # topology.py:129-131
-            if isinstance(conn, MaxPool2dConnection):
+            if isinstance(conn, _MaxPoolConnection):
                 raise AttributeError(conn._no_w_message())                              # self.w.masked_fill_, topology.py:127-131
             if hasattr(conn, "pipeline"):
                 continue                                  # MulticompartmentConnection.update ignores the kwarg (topology.py:509-518)
@@ -320,11 +320,11 @@ class Network(torch.nn.Module):
     def _launch(self, net, opts, dev) -> None:
         for layer in self.layers.values():
             _backend.require_cuda(layer.s, "layer state")
-        from .topology import MaxPool2dConnection
+        from .topology import _MaxPoolConnection
 
         for conn in self.connections.values():
-            if isinstance(conn, MaxPool2dConnection):
-                _backend.require_cuda(conn.firing_rates, "MaxPool2dConnection.firing_rates")
+            if isinstance(conn, _MaxPoolConnection):
+                _backend.require_cuda(conn.firing_rates, f"{type(conn).__name__}.firing_rates")
             else:
                 _backend.require_cuda(conn.w, "connection weights")
         try:
@@ -382,7 +382,7 @@ class Network(torch.nn.Module):
                 return True
         builtin_conns = (Tp.Connection, Tp.MulticompartmentConnection, Tp.Conv2dConnection, Tp.LocalConnection, Tp.SparseConnection,
                          Tp.MaxPool2dConnection, Tp.LocalConnection2D, Tp.Conv3dConnection, Tp.Conv1dConnection,
-                         Tp.LocalConnection3D)
+                         Tp.LocalConnection3D, Tp.MaxPoo3dConnection)
         for conn in self.connections.values():
             if type(conn) not in builtin_conns:
                 return True

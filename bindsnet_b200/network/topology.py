@@ -861,7 +861,44 @@ class SparseConnection(Connection):
         d.norm_abs = 0
 
 
-class MaxPool2dConnection(AbstractConnection):
+class _MaxPoolConnection(AbstractConnection):
+    """What MaxPool2dConnection and MaxPoo3dConnection share: no weights, the ``firing_rates`` buffer, the single
+    operator, and the reference's failures of ``NoOp.update`` and of ``masks=`` on a connection without ``w``."""
+
+    def compute(self, s: torch.Tensor) -> torch.Tensor:
+        """topology.py:1163-1185 / :1255-1277: ``firing_rates`` advance in place; returns the pooled spikes ``[B, C,
+        *pooled]`` (``snn_b200_conn_compute``)."""
+        from . import _plan
+
+        return _plan.compute_single_connection(self, s)
+
+    def update(self, **kwargs) -> None:
+        """topology.py:1187-1192 / :1279-1284 -> :112-139: with learning on, learning.NoOp.update reads ``self.w``; so
+        does a mask."""
+        if kwargs.get("learning", True) or kwargs.get("mask", None) is not None:
+            raise AttributeError(self._no_w_message())
+
+    def normalize(self) -> None:
+        """No weights, no normalization (topology.py:1194-1199)."""
+
+    def reset_state_variables(self) -> None:
+        """topology.py:1201-1211 / :1293-1301 (the reference allocates on the CPU; here the buffer stays on its device)."""
+        self.firing_rates = torch.zeros(self.source.batch_size, *self.source.s.shape[1:], device=self.firing_rates.device)
+
+    def _no_w_message(self) -> str:
+        name = _pool_dims(self)[1]
+        return (f"'{name}' object has no attribute 'w' (the reference's learning.NoOp.update and the masks= of "
+                f"Network.run read connection.w, learning.py:87-94 / topology.py:127-131; run {name} networks with "
+                "learning off and without masks for it)")
+
+    def _out_shape(self):
+        return pool_out_shape(self)
+
+    def _check(self, s_shape) -> None:
+        check_pool(self, s_shape)
+
+
+class MaxPool2dConnection(_MaxPoolConnection):
     """Max pooling by online firing-rate estimates (reference: topology.py:1124-1211).  Each ``compute(s)`` decays the
     ``firing_rates`` buffer (``r -= decay * r``), adds the spikes, and passes on, per channel and window, the spike of
     the source neuron with the highest rate (the first one in row-major window order on a tie; padding never wins).
@@ -885,36 +922,6 @@ class MaxPool2dConnection(AbstractConnection):
         self.dilation = _pair(dilation)
         self.register_buffer("firing_rates", torch.zeros(source.s.shape))
 
-    def compute(self, s: torch.Tensor) -> torch.Tensor:
-        """topology.py:1163-1185: ``firing_rates`` advance in place; returns the pooled spikes ``[B, C, Hout, Wout]``
-        (``snn_b200_conn_compute``)."""
-        from . import _plan
-
-        return _plan.compute_single_connection(self, s)
-
-    def update(self, **kwargs) -> None:
-        """topology.py:1187-1192 -> :112-139: with learning on, learning.NoOp.update reads ``self.w``; so does a mask."""
-        if kwargs.get("learning", True) or kwargs.get("mask", None) is not None:
-            raise AttributeError(self._no_w_message())
-
-    def normalize(self) -> None:
-        """No weights, no normalization (topology.py:1194-1199)."""
-
-    def reset_state_variables(self) -> None:
-        """topology.py:1201-1211 (the reference allocates on the CPU; here the buffer stays on its device)."""
-        self.firing_rates = torch.zeros(self.source.batch_size, *self.source.s.shape[1:], device=self.firing_rates.device)
-
-    def _no_w_message(self) -> str:
-        return ("'MaxPool2dConnection' object has no attribute 'w' (the reference's learning.NoOp.update and the masks= of "
-                "Network.run read connection.w, learning.py:87-94 / topology.py:127-131; run MaxPool2dConnection networks with "
-                "learning off and without masks for it)")
-
-    def _out_shape(self):
-        return pool_out_shape(self)
-
-    def _check(self, s_shape) -> None:
-        check_pool(self, s_shape)
-
     def _fill_desc(self, d: "_abi.SnnConn", dt: float, rule: bool = True) -> None:
         d.kind = _abi.SNN_CONN_MAXPOOL2D
         d.rule = _abi.SNN_RULE_NOOP
@@ -927,6 +934,56 @@ class MaxPool2dConnection(AbstractConnection):
         d.dh, d.dw = self.dilation
         d.pool_decay = float(np.float32(float(self.decay))) if self.decay is not None else 0.0
         d.pool_rates = self.firing_rates.data_ptr()
+
+
+class MaxPoo3dConnection(_MaxPoolConnection):
+    """Three-dimensional max pooling by online firing-rate estimates (reference: topology.py:1214-1301; the reference's
+    class name, typo included).  Each ``compute(s)`` decays the ``firing_rates`` buffer (``r -= decay * r``), adds the
+    spikes, and passes on, per channel and window, the spike of the source neuron with the highest rate (the first one
+    in ``(d, h, w)`` row-major window order on a tie; padding never wins).  Source and target are ``[C, D, H, W]``
+    populations with the target ``[C, Dout, Hout, Wout]`` as ``F.max_pool3d`` computes it; ``kernel_size``, ``stride``,
+    ``padding`` and ``dilation`` are ``(D, H, W)`` triples.  There are no weights and nothing to learn: the rule is
+    ``learning.NoOp``, ``normalize`` does nothing.
+
+    As in the reference, ``decay`` is a keyword argument without default, ``firing_rates`` is ``source.s.shape`` at
+    construction and ``reset_state_variables`` reallocates it at the source's batch size (here on the buffer's device).
+    Inside ``Network.run`` the generic window kernel keeps the rates in step with the reference's call order; the
+    reference's failures are raised before anything runs, with its exception types: ``RuntimeError`` for shapes its
+    ``fr += s.float().squeeze()`` cannot add (a size-1 dimension at batch size > 1, a buffer of another batch size), a
+    target that is not ``[C, Dout, Hout, Wout]``, padding above half the kernel and a window that lies entirely in the
+    padding; ``AttributeError`` for a learning window or ``masks=`` for it.  Unlike the reference, a source that is not a
+    population of shape ``[C, D, H, W]`` raises ``NotImplementedError`` at construction."""
+
+    def __init__(self, source: Nodes, target: Nodes, kernel_size, stride=1, padding=0, dilation=1, **kwargs) -> None:
+        if not isinstance(source, Nodes) or len(source.shape) != 4:
+            shape = list(source.shape) if isinstance(source, Nodes) else type(source).__name__
+            raise NotImplementedError(f"MaxPoo3dConnection is built from a [C, D, H, W] source population only; the source "
+                                      f"is {shape}")
+        super().__init__(source, target, None, None, 0.0, **kwargs)
+        self.kernel_size = _triple(kernel_size)
+        self.stride = _triple(stride)
+        self.padding = _triple(padding)
+        self.dilation = _triple(dilation)
+        self.register_buffer("firing_rates", torch.zeros(source.s.shape))
+
+    def _fill_desc(self, d: "_abi.SnnConn", dt: float, rule: bool = True) -> None:
+        d.kind = _abi.SNN_CONN_MAXPOOL3D
+        d.rule = _abi.SNN_RULE_NOOP
+        d.weight_decay = 1.0
+        fill_pool3d_geometry(d, self)
+        d.pool_decay = float(np.float32(float(self.decay))) if self.decay is not None else 0.0
+        d.pool_rates = self.firing_rates.data_ptr()
+
+
+def fill_pool3d_geometry(d: "_abi.SnnConn", conn) -> None:
+    """The SNN_CONN_MAXPOOL3D geometry of a MaxPoo3dConnection (this package's or the reference's: the same attributes):
+    the depth axis in the depth fields, H and W in the conv fields, ``cin = cout = C``."""
+    d.cin, d.din, d.hin, d.win = (int(v) for v in conn.source.shape)
+    d.cout, d.dout, d.hout, d.wout = pool_out_shape(conn)
+    d.kd, d.kh, d.kw = (int(v) for v in conn.kernel_size)
+    d.sd, d.sh, d.sw = (int(v) for v in conn.stride)
+    d.pd, d.ph, d.pw = (int(v) for v in conn.padding)
+    d.dd, d.dh, d.dw = (int(v) for v in conn.dilation)
 
 
 class LocalConnection2D(AbstractConnection):
@@ -1135,41 +1192,53 @@ def fill_local3d_geometry(d: "_abi.SnnConn", conn) -> None:
     d.dh = d.dw = 1
 
 
+def _pool_dims(conn):
+    """The number of spatial axes of a pooling connection (2 or 3: its kernel_size is a pair or a triple), the class
+    name and the pooling function its messages name."""
+    nd = len(conn.kernel_size)
+    return nd, ("MaxPool2dConnection" if nd == 2 else "MaxPoo3dConnection"), f"max_pool{nd}d"
+
+
 def pool_out_shape(conn):
-    """``[C, Hout, Wout]`` of a MaxPool2dConnection (this package's or the reference's: the same attributes), or the
-    ``RuntimeError`` the reference's ``compute`` raises for its geometry.  ``F.max_pool2d`` without ceil mode; every window
-    must hold an element of the image (a dilated window can lie entirely in the padding, where the reference's gather
-    indexes past the row)."""
+    """``[C, Hout, Wout]`` of a MaxPool2dConnection, ``[C, Dout, Hout, Wout]`` of a MaxPoo3dConnection (this package's or
+    the reference's: the same attributes), or the ``RuntimeError`` the reference's ``compute`` raises for its geometry.
+    ``F.max_pool2d`` / ``F.max_pool3d`` without ceil mode; every window must hold an element of the input on every axis (a
+    dilated window can lie entirely in the padding, where the reference's gather indexes past the row)."""
+    nd, name, fn = _pool_dims(conn)
     shape = tuple(int(v) for v in conn.source.shape)
-    if len(shape) != 3:
-        raise RuntimeError(f"MaxPool2dConnection needs a [C, H, W] source population, got {list(shape)} (the reference's "
+    if len(shape) != nd + 1:
+        axes = "[C, H, W]" if nd == 2 else "[C, D, H, W]"
+        raise RuntimeError(f"{name} needs a {axes} source population, got {list(shape)} (the reference's "
                            "gather over s.flatten(2) indexes the wrong dimension)")
     out = []
     for n, k, st, p, d in zip(shape[1:], conn.kernel_size, conn.stride, conn.padding, conn.dilation):
         if k < 1 or st < 1 or d < 1 or p < 0:
-            raise RuntimeError(f"max_pool2d: kernel_size {conn.kernel_size}, stride {conn.stride} and dilation {conn.dilation} must be "
+            raise RuntimeError(f"{fn}: kernel_size {conn.kernel_size}, stride {conn.stride} and dilation {conn.dilation} must be "
                                f"positive and padding {conn.padding} non-negative")
         if p > k // 2:
             raise RuntimeError(f"pad should be at most half of effective kernel size, but got pad={p}, kernel_size={k} and dilation={d}")
         e = n + 2 * p - d * (k - 1) - 1
         if e < 0:
-            raise RuntimeError(f"max_pool2d: output size is too small for input {list(shape)}")
+            raise RuntimeError(f"{fn}: output size is too small for input {list(shape)}")
         m = e // st + 1
         for o in range(m):
             if not any(0 <= o * st - p + j * d < n for j in range(k)):
-                raise RuntimeError(f"max_pool2d: window {o} of kernel_size {k}, stride {st}, padding {p} and dilation {d} lies "
+                raise RuntimeError(f"{fn}: window {o} of kernel_size {k}, stride {st}, padding {p} and dilation {d} lies "
                                    f"entirely in the padding of a dimension of size {n}")
         out.append(m)
-    return shape[0], out[0], out[1]
+    return (shape[0], *out)
 
 
 def check_pool(conn, s_shape) -> None:
-    """The conditions under which the reference's ``MaxPool2dConnection.compute`` on spikes of shape ``s_shape`` succeeds,
-    raised as it raises: ``decay`` set, a buffer that ``fr += s.float().squeeze()`` adds to element by element (the same
-    shape as ``s``), a geometry ``pool_out_shape`` accepts, a target of the pooled shape."""
+    """The conditions under which the reference's ``MaxPool2dConnection.compute`` / ``MaxPoo3dConnection.compute`` on
+    spikes of shape ``s_shape`` succeeds, raised as it raises: ``decay`` set, a buffer that ``fr += s.float().squeeze()``
+    adds to element by element (the same shape as ``s``), a geometry ``pool_out_shape`` accepts, a target of the pooled
+    shape."""
+    nd, name, _ = _pool_dims(conn)
+    line = 1175 if nd == 2 else 1265
     if conn.decay is None:
-        raise TypeError("unsupported operand type(s) for *: 'NoneType' and 'Tensor' (MaxPool2dConnection needs the decay= "
-                        "keyword argument, topology.py:1175)")
+        raise TypeError(f"unsupported operand type(s) for *: 'NoneType' and 'Tensor' ({name} needs the decay= "
+                        f"keyword argument, topology.py:{line})")
     fr = tuple(conn.firing_rates.shape)
     sq = tuple(d for d in s_shape if d != 1)
     try:
@@ -1178,16 +1247,17 @@ def check_pool(conn, s_shape) -> None:
         ok = False
     if not ok or fr != tuple(s_shape):
         raise RuntimeError(
-            f"MaxPool2dConnection: firing_rates of shape {list(fr)} cannot take the spikes of shape {list(s_shape)} the way "
-            "the reference adds them (firing_rates += s.float().squeeze(), topology.py:1176); call reset_state_variables() "
+            f"{name}: firing_rates of shape {list(fr)} cannot take the spikes of shape {list(s_shape)} the way "
+            f"the reference adds them (firing_rates += s.float().squeeze(), topology.py:{line + 1}); call reset_state_variables() "
             "after the batch size changes, and note that a size-1 channel or spatial dimension at batch size > 1 fails "
             "in the reference too")
     out = pool_out_shape(conn)
     if tuple(int(v) for v in conn.target.shape) != out:
-        raise RuntimeError(f"MaxPool2dConnection: target shape {list(conn.target.shape)} is not the pooled shape {list(out)} "
-                           "(network.py:248 adds [B, C, Hout, Wout] into it)")
+        pooled = "[B, C, Hout, Wout]" if nd == 2 else "[B, C, Dout, Hout, Wout]"
+        raise RuntimeError(f"{name}: target shape {list(conn.target.shape)} is not the pooled shape {list(out)} "
+                           f"(network.py:248 adds {pooled} into it)")
     if conn.firing_rates.dtype != torch.float32 or not conn.firing_rates.is_contiguous():
-        raise TypeError("MaxPool2dConnection.firing_rates must be a contiguous float32 tensor (it is updated in place)")
+        raise TypeError(f"{name}.firing_rates must be a contiguous float32 tensor (it is updated in place)")
 
 
 def _unsupported(name: str, where: str):
@@ -1205,6 +1275,5 @@ def _unsupported(name: str, where: str):
 
 
 MaxPool1dConnection = _unsupported("MaxPool1dConnection", "topology.py:1028-1121")
-MaxPoo3dConnection = _unsupported("MaxPoo3dConnection", "topology.py:1214-1301")
 LocalConnection1D = _unsupported("LocalConnection1D", "topology.py:1487-1620")
 MeanFieldConnection = _unsupported("MeanFieldConnection", "topology.py:1920-2006")

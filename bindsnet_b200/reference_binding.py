@@ -11,7 +11,8 @@ Covered: what ``bindsnet.models`` builds for the hot path — ``Input`` / ``LIFN
 ``MulticompartmentConnection`` with one ``Weight`` feature (``MCC_learning.NoOp`` / ``PostPre``) and the classic
 ``Connection``, ``LocalConnection2D`` and ``LocalConnection3D`` with ``learning.NoOp`` / ``PostPre`` / ``WeightDependentPostPre`` / ``Hebbian``,
 ``Conv3dConnection`` with the updates the reference can run on it, ``Conv1dConnection`` with ``learning.NoOp`` /
-``PostPre`` / ``WeightDependentPostPre`` / ``Hebbian``.  Every attribute is read where the
+``PostPre`` / ``WeightDependentPostPre`` / ``Hebbian``, ``MaxPool2dConnection`` and ``MaxPoo3dConnection`` with learning off.
+Every attribute is read where the
 reference keeps it (file:line in the comments); state tensors are handed over by pointer and updated in place.
 """
 from __future__ import annotations
@@ -133,29 +134,34 @@ def _neuron_rows(layer, kind: int) -> Dict[str, tuple]:
 def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep: Optional[List[torch.Tensor]] = None,
                     B: Optional[int] = None, device: Optional[torch.device] = None) -> None:
     """``B`` / ``device``: the run's batch size and the layers' device (default: the source layer's), against which a
-    MaxPool2dConnection's rates buffer is checked."""
+    MaxPool2dConnection's or MaxPoo3dConnection's rates buffer is checked."""
     keep = keep if keep is not None else []
     d.src, d.tgt = src, tgt
     d.weight_decay, d.dt_scale = 1.0, 1.0
-    if type(conn).__name__ == "MaxPool2dConnection":
-        # topology.py:1124-1211: no weights; the firing_rates buffer is updated in place, so it must be [B, *source.shape]
+    if type(conn).__name__ in ("MaxPool2dConnection", "MaxPoo3dConnection"):
+        # topology.py:1124-1301: no weights; the firing_rates buffer is updated in place, so it must be [B, *source.shape]
         # for this run (the window reads and writes B * n_src floats) and on the run's device.  The reference allocates it
         # on the CPU at reset_state_variables (:1209-1211) and never resizes it when the batch size changes: move it to the
         # layers' device and reset it after a batch change before binding a run.
-        from .network.topology import check_pool, pool_out_shape
+        from .network.topology import check_pool, fill_pool3d_geometry, pool_out_shape
 
         B = int(conn.source.s.shape[0]) if B is None else int(B)
         device = conn.source.s.device if device is None else torch.device(device)
         check_pool(conn, (B, *conn.source.shape))   # the reference's RuntimeError / TypeError, raised before anything runs
         fr = conn.firing_rates
         if fr.device != device:
-            raise RuntimeError(f"MaxPool2dConnection.firing_rates is on {fr.device}, the run on {device}: move it to the "
+            raise RuntimeError(f"{type(conn).__name__}.firing_rates is on {fr.device}, the run on {device}: move it to the "
                                "layers' device first")
-        d.kind, d.rule = _abi.SNN_CONN_MAXPOOL2D, _abi.SNN_RULE_NOOP
-        d.cin, d.hin, d.win = (int(v) for v in conn.source.shape)
-        d.cout, d.hout, d.wout = pool_out_shape(conn)
-        (d.kh, d.kw), (d.sh, d.sw) = conn.kernel_size, conn.stride
-        (d.ph, d.pw), (d.dh, d.dw) = conn.padding, conn.dilation
+        d.rule = _abi.SNN_RULE_NOOP
+        if type(conn).__name__ == "MaxPoo3dConnection":
+            d.kind = _abi.SNN_CONN_MAXPOOL3D
+            fill_pool3d_geometry(d, conn)
+        else:
+            d.kind = _abi.SNN_CONN_MAXPOOL2D
+            d.cin, d.hin, d.win = (int(v) for v in conn.source.shape)
+            d.cout, d.hout, d.wout = pool_out_shape(conn)
+            (d.kh, d.kw), (d.sh, d.sw) = conn.kernel_size, conn.stride
+            (d.ph, d.pw), (d.dh, d.dw) = conn.padding, conn.dilation
         d.pool_decay = _f(conn.decay)
         d.pool_rates = fr.data_ptr()
         return
@@ -424,10 +430,10 @@ def build_net(network, inputs: Dict[str, torch.Tensor], T: int, B: int):
     dev = next(iter(network.layers.values())).s.device
     layers = list(network.layers.values())
     for i, ((s, t), conn) in enumerate(network.connections.items()):
-        if network.learning and type(conn).__name__ == "MaxPool2dConnection":
+        if network.learning and type(conn).__name__ in ("MaxPool2dConnection", "MaxPoo3dConnection"):
             # the reference fails in the first step's update: learning.NoOp.update scales connection.w (learning.py:87-94)
-            raise AttributeError("'MaxPool2dConnection' object has no attribute 'w' (run MaxPool2dConnection networks with "
-                                 "learning off)")
+            name = type(conn).__name__
+            raise AttributeError(f"'{name}' object has no attribute 'w' (run {name} networks with learning off)")
         if network.learning and type(conn).__name__ == "Conv3dConnection":
             rule = conn.update_rule
             name = type(rule).__name__

@@ -178,7 +178,23 @@ extern "C" {
                               norm / (its sum, ascending k), no guard against a zero sum.  No mask.  Generic tier only,
                               not with SNN_CONN_SPARSE, MCC features or per-neuron parameters; a library older than the
                               kind refuses it with SNN_ERR_UNSUPPORTED */
-#define SNN_RULE_NONE 0        /* MCC_learning.NoOp: update() does nothing    MCC_learning.py:120-146 */
+#define SNN_CONN_MAXPOOL3D 9 /* MaxPoo3dConnection: online-rate 3-D max pooling, topology.py:1214-1301.  No weights (w, b,
+                                norm and mask absent), rule SNN_RULE_NOOP only.  Source [C,din,hin,win], target
+                                [C,dout,hout,wout], both row-major: the H and W axes in the conv fields as on
+                                SNN_CONN_MAXPOOL2D (cin = cout = C; kh/kw, sh/sw, ph/pw, dh/dw), the depth axis in
+                                din, dout, kd, sd, pd, dd (the fields SNN_CONN_CONV3D overlays on the sparse storage),
+                                each as for F.max_pool3d without ceil mode: padding at most half the kernel, and every
+                                window holds an element of the volume on every axis.  Each compute:
+                                  1. r = fl(r - fl(pool_decay * r)); r = fl(r + s)   on pool_rates [B,C,din,hin,win]
+                                  2. idx = the first maximum of r[b,c] over the window in (kz, ky, kx) row-major order,
+                                     padding never chosen (strict >, so -0 == +0 ties keep the earlier element; a NaN
+                                     takes over)
+                                  3. out[b,c,oz,oy,ox] = s[b,c,idx] as 0.0 / 1.0
+                                The rates a step reads fold in the spikes that step's gather reads, as on
+                                SNN_CONN_MAXPOOL2D.  Generic tier only; not in a plan that also holds an SNN_CONN_SPARSE
+                                connection, MCC features or per-neuron parameters, and never into a PassThroughNodes
+                                layer; a library older than the kind refuses it with SNN_ERR_UNSUPPORTED */
+#define SNN_RULE_NONE 0       /* MCC_learning.NoOp: update() does nothing    MCC_learning.py:120-146 */
 #define SNN_RULE_NOOP 1        /* learning.NoOp: weight decay only, no clamp  learning.py:107-146     */
 #define SNN_RULE_POSTPRE 2     /* learning.PostPre._connection_update         learning.py:390-420     */
 #define SNN_RULE_WDEP_POSTPRE 3/* learning.WeightDependentPostPre             learning.py:626-653     */
@@ -338,7 +354,8 @@ typedef struct snn_conn {
        [0, nnz]; sp_col [nnz], strictly ascending within a row, < n_tgt; w [nnz] the values in the same order, decayed
        in place by SNN_RULE_NOOP.  A malformed pattern is reported as SNN_ERR_BAD_ARG (in *err_flag by the window).
        SNN_CONN_CONV3D (topology.py:847-1025) keeps its depth axis in the same storage: source depth din, target depth
-       dout, kernel depth kd, stride sd, padding pd.  A connection is never both, so the layout is the one without it. */
+       dout, kernel depth kd, stride sd, padding pd; SNN_CONN_MAXPOOL3D also its depth dilation dd (read by no other
+       kind).  A connection is never both, so the layout is the one without it. */
     union {
         struct {
             const int32_t *sp_rowptr;
@@ -346,7 +363,7 @@ typedef struct snn_conn {
             int32_t nnz;
         };
         struct {
-            int32_t din, dout, kd, sd, pd;
+            int32_t din, dout, kd, sd, pd, dd;
         };
     };
     /* SNN_CONN_MCC with Probability / Mask / Intensity features besides its Weight (topology.py:437-479).  Each is an
@@ -387,7 +404,8 @@ typedef struct snn_conn {
             int8_t wmin_form, wmax_form, nu0_form, nu1_form;
         };
     };
-    /* SNN_CONN_MAXPOOL2D (topology.py:1124-1211): the firing_rates buffer [B, C, hin, win], updated in place (after a
+    /* SNN_CONN_MAXPOOL2D (topology.py:1124-1211) and SNN_CONN_MAXPOOL3D (:1214-1301): the firing_rates buffer
+       [B, C, hin, win] (3-D: [B, C, din, hin, win]), updated in place (after a
        window it holds what the reference's buffer holds after the window's last compute), and the decay kwarg rounded
        to fp32 as `decay * firing_rates` rounds it. */
     float *pool_rates;

@@ -79,7 +79,11 @@ static int validate(const snn_net_t *net, const snn_run_opts_t *o) {
         if (pool ? (C.w || C.b) : (!C.w && !(sparse && C.nnz == 0))) return SNN_ERR_BAD_ARG;
         if (net->layers[C.tgt].kind == SNN_NODE_INPUT) return SNN_ERR_UNSUPPORTED;
         if (C.rule < SNN_RULE_NONE || C.rule > SNN_RULE_MSTDPET) return SNN_ERR_UNSUPPORTED;
-        if (C.kind < SNN_CONN_DENSE || C.kind > SNN_CONN_MAXPOOL3D) return SNN_ERR_UNSUPPORTED;
+        if (C.kind < SNN_CONN_DENSE || C.kind > SNN_CONN_MEANFIELD) return SNN_ERR_UNSUPPORTED;
+        if (C.kind == SNN_CONN_MEANFIELD) {   // w is only read; the mean is exact below 2^24 spikes (snn_b200.h)
+            if (!C.mf_off || C.b || C.mf_stride < 0 || (long long)o->B * net->layers[C.src].n >= (1LL << 24)) return SNN_ERR_BAD_ARG;
+            if ((C.rule != SNN_RULE_NONE && C.rule != SNN_RULE_NOOP) || C.has_norm || C.mask) return SNN_ERR_UNSUPPORTED;
+        }
         if (conv1d) {   // NoOp and the three unsupervised rules, no mask (snn_b200.h)
             const int rc = snn_conv1d_geometry_ok(C, net->layers[C.src].n, net->layers[C.tgt].n);
             if (rc != SNN_OK) return rc;
@@ -157,6 +161,13 @@ static bool has_pool(const snn_net_t *net) {
     return false;
 }
 
+// some connection is a MeanFieldConnection: every generic instantiation runs it, the fused kernels do not
+static bool has_meanfield(const snn_net_t *net) {
+    for (int c = 0; c < net->n_conns; ++c)
+        if (net->conns[c].kind == SNN_CONN_MEANFIELD) return true;
+    return false;
+}
+
 static bool has_sparse(const snn_net_t *net) {
     for (int c = 0; c < net->n_conns; ++c)
         if (net->conns[c].kind == SNN_CONN_SPARSE) return true;
@@ -191,8 +202,10 @@ static bool layer_needs_xpub(const snn_net_t *net, int l) {
 static size_t layout_generic(const snn_net_t *net, const snn_run_opts_t *o, char *ws, DevNet *N) {
     size_t off = 0;
     const size_t B = (size_t)o->B;
+    // the barrier counters, then the spike-count slots of the MeanFieldConnection sources (layer l: words
+    // SNN_BAR_WORDS + 3 l ..., on a cache line of their own); the launch zeroes both
     if (N) N->bar = (unsigned int *)(ws + off);
-    off += align_up(sizeof(unsigned int) * 96);
+    off += align_up(sizeof(unsigned int) * SNN_BAR_ZERO_WORDS);
     int items = 0;
     for (int l = 0; l < net->n_layers; ++l) {
         const snn_layer_t &L = net->layers[l];
@@ -216,8 +229,12 @@ static size_t layout_generic(const snn_net_t *net, const snn_run_opts_t *o, char
         if (th) off += align_up(sizeof(int32_t) * 3 * L.n);
         bool wide_src = false;   // source of a dense connection with more than one gather block
         for (int c = 0; c < net->n_conns; ++c)
-            if (net->conns[c].src == l && net->conns[c].kind != SNN_CONN_CONV2D && !snn_pool_inst_kind(net->conns[c].kind) && nw > 32)
+            if (net->conns[c].src == l && net->conns[c].kind != SNN_CONN_CONV2D && net->conns[c].kind != SNN_CONN_MEANFIELD &&
+                !snn_pool_inst_kind(net->conns[c].kind) && nw > 32)
                 wide_src = true;
+        bool mf_src = false;
+        for (int c = 0; c < net->n_conns; ++c) mf_src |= net->conns[c].src == l && net->conns[c].kind == SNN_CONN_MEANFIELD;
+        if (N) N->layers[l].spc = mf_src ? (int32_t *)(N->bar + SNN_BAR_WORDS + 3 * l) : nullptr;
         if (N) N->layers[l].anyf = wide_src ? (uint32_t *)(ws + off) : nullptr;
         if (wide_src) off += align_up(sizeof(uint32_t) * 3 * B);
         if (N && os) N->any_one_spike = 1;
@@ -284,9 +301,9 @@ static int select_tier(const snn_net_t *net, const snn_run_opts_t *opts, bool pn
         if (has_sparse(net) || has_feat(net) || has_pool(net)) return 0;
         return (opts->tier == 0 || opts->tier == 1) && !opts->delta_w && !opts->delta_theta ? 1 : 0;
     }
-    // the fused DiehlAndCook2015 kernels (and so the delta windows) have neither the sparse, the feature nor the pooling
-    // gather, and read scalar bounds and rates only
-    if (has_sparse(net) || has_feat(net) || has_pool(net) || has_syn(net))
+    // the fused DiehlAndCook2015 kernels (and so the delta windows) have neither the sparse, the feature, the pooling
+    // nor the mean-field gather, and read scalar bounds and rates only
+    if (has_sparse(net) || has_feat(net) || has_pool(net) || has_syn(net) || has_meanfield(net))
         return (opts->tier == 0 || opts->tier == 1) && !opts->delta_w && !opts->delta_theta ? 1 : 0;
     if (opts->delta_w || opts->delta_theta)   // delta windows exist in the barrier kernel only
         return (opts->tier == 0 || opts->tier == 2) && snn_fused_dc_supported(net, opts) ? 2 : 0;
@@ -314,7 +331,7 @@ size_t snn_b200_workspace_bytes(const snn_net_t *net0, const snn_run_opts_t *opt
     const snn_net_t *net = &P;
     if (validate(net, opts) != SNN_OK) return 0;
     size_t g = layout_generic(net, opts, nullptr, nullptr);
-    if (pn || has_sparse(net) || has_feat(net) || has_pool(net) || has_syn(net)) return g;
+    if (pn || has_sparse(net) || has_feat(net) || has_pool(net) || has_syn(net) || has_meanfield(net)) return g;
     size_t f = snn_fused_dc_supported(net, opts) ? snn_fused_dc_workspace_bytes(net, opts) : 0;
     size_t f2 = snn_fused_dc2_supported(net, opts) ? snn_fused_dc2_workspace_bytes(net, opts) : 0;
     if (f2 > f) f = f2;
@@ -359,7 +376,7 @@ int snn_b200_run_window(const snn_net_t *net0, const snn_run_opts_t *opts, void 
         if (C.kind == SNN_CONN_MCC && (C.f_prob || C.f_mask || C.f_int)) N.any_feat = 1;
     }
     N.any_pool = has_pool(net) ? 1 : 0;
-    if (cudaMemsetAsync(N.bar, 0, sizeof(unsigned int) * 96, stream) != cudaSuccess) return SNN_ERR_CUDA;
+    if (cudaMemsetAsync(N.bar, 0, sizeof(unsigned int) * SNN_BAR_ZERO_WORDS, stream) != cudaSuccess) return SNN_ERR_CUDA;
     const int e = snn_generic_launch(N, stream);
     if (e != 0) {
         fprintf(stderr, "libsnn_b200: generic window launch failed: %s\n", cudaGetErrorString((cudaError_t)e));

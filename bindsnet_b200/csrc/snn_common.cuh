@@ -34,6 +34,11 @@
 #define SNN_GEN_THREADS 256  // generic kernel: 8 warps per CTA
 #define SNN_GEN_WARPS (SNN_GEN_THREADS / 32)
 
+// The generic window's barrier block: SNN_BAR_WORDS counter words, then three spike-count slots per layer (DevLayer::spc),
+// all zeroed before every launch.
+#define SNN_BAR_WORDS 96
+#define SNN_BAR_ZERO_WORDS (SNN_BAR_WORDS + 3 * SNN_MAX_LAYERS)
+
 struct DevLayer {
     snn_layer_t L;
     uint32_t *bits;             // [2][B][nw]  bit-packed spikes, slot t&1 holds s(t)
@@ -44,6 +49,8 @@ struct DevLayer {
     int32_t *thcnt;             // [3][n]      DC: threshold crossers of step t summed over the batch (slot t%3)
     uint32_t *anyf;             // [3][B]      wide source layers (nw > 32) of dense connections: non-zero iff the sample spiked
                                 //             in step t (slot t%3) — lets a gather skip an all-zero bit row without reading it
+    int32_t *spc;               // [3]         source of a MeanFieldConnection: the spikes of step t counted over the
+                                //             batch and the layer (slot t%3); NULL for every other layer
     int32_t nw;                 // ceil(n / 32)
     int32_t item0;              // first work-item index of this layer
 };

@@ -1,6 +1,6 @@
 // snn_generic.cu — generic persistent window kernel (any topology of Input / McCullochPitts / IF / LIF / BoostedLIF /
 // CurrentLIF / DiehlAndCook / SubtractiveResetIF / PassThrough populations joined by dense, convolutional, sparse,
-// pooling and 2-D and 3-D locally connected connections).
+// pooling, 2-D and 3-D locally connected and mean-field connections).
 //
 // One cooperative grid iterates the whole T-step window of Network.run (reference:
 // bindsnet/network/network.py:380-465) with at most four grid barriers per step and no host involvement.
@@ -85,12 +85,15 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
         int li, tile; item_of(N, item, li, tile);
         const DevLayer &D = N.layers[li];
         const int j = tile * SNN_TILE + lane;
+        int nsp = 0;   // (a MeanFieldConnection source) s(-1) counted into slot 2, the slot of step -1
         for (int b = warp; b < N.B; b += SNN_GEN_WARPS) {
             const size_t k = (size_t)b * D.L.n + j;
             const bool s = j < D.L.n && (POOL && D.L.kind == SNN_NODE_PASSTHROUGH ? passthrough_spike(D.L, k, N.err) : D.L.s[k] != 0);
             const uint32_t w = __ballot_sync(0xffffffffu, s);
             if (lane == 0) D.bits[((size_t)1 * N.B + b) * D.nw + tile] = w;
+            nsp += __popc(w);
         }
+        if (D.spc && lane == 0 && nsp) atomicAdd(D.spc + 2, nsp);
         if (D.keys && tile == 0)
             for (int b = threadIdx.x; b < 2 * N.B; b += blockDim.x) D.keys[b] = 0ull;
         if (D.thcnt && warp < 3 && j < D.L.n) D.thcnt[(size_t)warp * D.L.n + j] = 0;
@@ -286,8 +289,10 @@ static int plan_units(DevNet &N, int cap) {
         const snn_conn_t &C = N.conns[c];
         N.p3_first[c] = p3;
         N.p3_rc[c] = 0;
-        if (!N.learning || C.rule == SNN_RULE_NONE || C.kind == SNN_CONN_CONV2D || C.kind == SNN_CONN_SPARSE || snn_pool_inst_kind(C.kind))
-            continue;   // (a pooling connection has no weights to update; conv and local rules are spread over the grid)
+        if (!N.learning || C.rule == SNN_RULE_NONE || C.kind == SNN_CONN_CONV2D || C.kind == SNN_CONN_SPARSE || snn_pool_inst_kind(C.kind) ||
+            C.kind == SNN_CONN_MEANFIELD)
+            continue;   // (a pooling connection has no weights to update, a mean-field one's NoOp leaves them as they are;
+                        // conv and local rules are spread over the grid)
         const int nwS = N.layers[C.src].nw, nwT = N.layers[C.tgt].nw;
         if (SNN_RULE_IS_MSTDP(C.rule)) { N.p3_rc[c] = 1; p3 += nwS; continue; }
         int rc = ceil_div(cap, nwT);

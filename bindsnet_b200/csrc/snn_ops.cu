@@ -316,6 +316,26 @@ __global__ void __launch_bounds__(256) verify_structure_kernel(const float *__re
     if (__syncthreads_or(bad) && threadIdx.x == 0 && err) atomicOr(err, SNN_ERR_STRUCTURE);
 }
 
+// MeanFieldConnection.compute (topology.py:1972-1981): out[b, j] = fl(fl(count / N) * w[mf_off[j] + b * mf_stride]), where
+// count is the number of spikes in the whole [B, n_src] tensor and N = B * n_src (snn_b200.h).  The count couples every
+// sample, so one CTA forms it (an integer: exact in any order) and then writes every output.
+__global__ void __launch_bounds__(1024) meanfield_compute_kernel(snn_conn_t C, int nt, int B, int N, const uint8_t *__restrict__ s,
+                                                                 float *__restrict__ out) {
+    SNN_SHARED(int, s_cnt, 1);
+    if (threadIdx.x == 0) s_cnt[0] = 0;
+    __syncthreads();
+    int c = 0;
+    for (int k = threadIdx.x; k < N; k += blockDim.x) c += s[k] != 0;
+    if (c) atomicAdd(s_cnt, c);
+    __syncthreads();
+    const float mean = (float)s_cnt[0] / (float)N;
+    const size_t total = (size_t)B * nt;
+    for (size_t k = threadIdx.x; k < total; k += blockDim.x) {
+        const int b = (int)(k / nt), j = (int)(k - (size_t)b * nt);
+        out[k] = mean * C.w[C.mf_off[j] + (size_t)b * C.mf_stride];
+    }
+}
+
 inline int cuda_rc(cudaError_t e) { return e == cudaSuccess ? SNN_OK : SNN_ERR_CUDA; }
 
 }  // namespace
@@ -346,6 +366,11 @@ int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, 
         const int blocks = (int)((tout + 255) / 256 < 4736 ? (tout + 255) / 256 : 4736);
         if (conn->kind == SNN_CONN_MAXPOOL3D) SNN_LAUNCH(pool_compute_kernel<true>, blocks, 256, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
         else SNN_LAUNCH(pool_compute_kernel<false>, blocks, 256, 0, (cudaStream_t)stream, *conn, n_src, n_tgt, B, s, out);
+        return cuda_rc(cudaGetLastError());
+    }
+    if (conn->kind == SNN_CONN_MEANFIELD) {   // the count over the batch is exact below 2^24 spikes (snn_b200.h)
+        if (!conn->mf_off || conn->b || conn->mf_stride < 0 || (long long)B * n_src >= (1LL << 24)) return SNN_ERR_BAD_ARG;
+        SNN_LAUNCH(meanfield_compute_kernel, 1, 1024, 0, (cudaStream_t)stream, *conn, n_tgt, B, B * n_src, s, out);
         return cuda_rc(cudaGetLastError());
     }
     if (conn->kind == SNN_CONN_LOCAL2D) {
@@ -415,6 +440,8 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
         return cuda_rc(cudaGetLastError());
     }
     if (!C.w) return SNN_ERR_BAD_ARG;
+    if (C.kind == SNN_CONN_MEANFIELD)   // learning.NoOp scales w by 1.0 and does not clamp: nothing changes (snn_b200.h)
+        return C.rule == SNN_RULE_NONE || C.rule == SNN_RULE_NOOP ? SNN_OK : SNN_ERR_UNSUPPORTED;
     if (C.kind == SNN_CONN_CONV3D) {   // decay / clamp only (snn_b200.h), dense over w
         const int rc = snn_conv3d_geometry_ok(C, net->layers[C.src].n, net->layers[C.tgt].n);
         if (rc != SNN_OK) return rc;
@@ -506,7 +533,8 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
 
 int snn_b200_conn_normalize(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, void *stream) {
     if (!conn || n_src <= 0 || n_tgt <= 0) return SNN_ERR_BAD_ARG;
-    if (conn->kind == SNN_CONN_SPARSE) return SNN_ERR_UNSUPPORTED;   // the reference's normalize fails on a sparse w too
+    // the reference's normalize fails on a sparse w, and on a mean-field one with norm set
+    if (conn->kind == SNN_CONN_SPARSE || (conn->kind == SNN_CONN_MEANFIELD && conn->has_norm)) return SNN_ERR_UNSUPPORTED;
     if (!conn->w) return SNN_ERR_BAD_ARG;
     if (!conn->has_norm) return SNN_OK;
     if (conn->kind == SNN_CONN_LOCAL2D) {   // rows of w viewed as [cin * n_tgt, K]

@@ -578,6 +578,10 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
     const bool deferred = dc && L.one_spike;  // final spikes known only after the arg-max
     bool nonbin = false;
 
+    // (a MeanFieldConnection source) the final spikes this warp publishes, counted by lane 0 and added to the layer's
+    // count of step t once per unit
+    int nsp = 0;
+    if (D.spc && tile == 0 && chunk == 0 && threadIdx.x == 0) D.spc[(t + 1) % 3] = 0;   // last read in step t - 1
     if (L.kind == SNN_NODE_INPUT) {
         // Input.forward (nodes.py:211-221): s = x.  Four samples per warp are in flight at once.
         for (int bb = b0 + warp; bb < b1; bb += 4 * SNN_GEN_WARPS) {
@@ -604,9 +608,11 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
                 if (lane == 0) {
                     D.bits[((size_t)wr * B + b) * nw + tile] = fw;
                     if (D.anyf && fw) atomicOr(D.anyf + (size_t)(t % 3) * B + b, 1u);
+                    if (D.spc) nsp += __popc(fw);
                 }
             }
         }
+        if (D.spc && nsp) atomicAdd(D.spc + t % 3, nsp);
         if (D.anyf && tile == 0)
             for (int b = b0 + threadIdx.x; b < b1; b += SNN_GEN_THREADS) D.anyf[(size_t)((t + 1) % 3) * B + b] = 0u;
         if (nonbin && N.err) atomicOr(N.err, SNN_ERR_NONBINARY);
@@ -696,8 +702,8 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
         #pragma unroll
         for (int q = 0; q < 4; ++q) {
             fwn[q] = 0u; afn[q] = 1u;
-            if (q < ncl && b < b1 && N.conns[cl[q]].kind != SNN_CONN_CONV2D && !(SPARSE && N.conns[cl[q]].kind == SNN_CONN_SPARSE) &&
-                !(POOL && snn_pool_inst_kind(N.conns[cl[q]].kind))) {
+            if (q < ncl && b < b1 && N.conns[cl[q]].kind != SNN_CONN_CONV2D && N.conns[cl[q]].kind != SNN_CONN_MEANFIELD &&
+                !(SPARSE && N.conns[cl[q]].kind == SNN_CONN_SPARSE) && !(POOL && snn_pool_inst_kind(N.conns[cl[q]].kind))) {
                 const snn_conn_t &C = N.conns[cl[q]];
                 const DevLayer &S = N.layers[C.src];
                 const int slot = (N.one_step && C.src < li) ? wr : rd;
@@ -780,6 +786,10 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
             } else if (POOL && C.kind == SNN_CONN_LOCAL3D) {
                 p = c == conv_c && st_bits ? gather_local2d<true, true>(C, M.cbits + (size_t)(b - b0) * S.nw, n, j, valid)
                                            : gather_local2d<false, true>(C, S.bits + ((size_t)slot * B + b) * S.nw, n, j, valid);
+            } else if (C.kind == SNN_CONN_MEANFIELD) {   // s.float().mean() * w (snn_b200.h): the source's count of the step
+                const int cnt_s = __ldcg(S.spc + (slot == wr ? t % 3 : (t + 2) % 3));
+                const float mean = (float)cnt_s / (float)(B * S.L.n);
+                p = valid ? mean * C.w[C.mf_off[j] + (size_t)b * C.mf_stride] : 0.0f;
             } else if (SPARSE && C.kind == SNN_CONN_SPARSE) {   // gathered by phase_sparse ahead of this phase
                 p = valid ? __ldcg(N.sp[c].out + (size_t)b * n + j) : 0.0f;
                 if (C.b && valid) p = p + C.b[j];
@@ -848,9 +858,11 @@ __device__ void phase1(const DevNet &N, int li, int tile, int chunk, int t, cons
             if (lane == 0) {
                 D.bits[((size_t)wr * B + b) * nw + tile] = fw;
                 if (D.anyf && fw) atomicOr(D.anyf + (size_t)(t % 3) * B + b, 1u);
+                if (D.spc) nsp += __popc(fw);
             }
         }
     }
+    if (D.spc && nsp) atomicAdd(D.spc + t % 3, nsp);
     if (D.anyf && tile == 0)   // the flag slot of step t + 1 (last read in step t - 1)
         for (int b = b0 + threadIdx.x; b < b1; b += SNN_GEN_THREADS) D.anyf[(size_t)((t + 1) % 3) * B + b] = 0u;
 
@@ -879,6 +891,7 @@ __device__ void phase2(const DevNet &N, int li, int tile, int chunk, int t) {
     if (PN) P = neuron_par(L, valid ? j : 0);
     const int wr = t & 1;
     const int b0 = chunk * N.cs, b1 = min(B, b0 + N.cs);
+    int nsp = 0;   // (a MeanFieldConnection source) the winners this warp publishes, as in phase 1
     for (int bb = b0 + warp; bb < b1; bb += 4 * SNN_GEN_WARPS) {
         uint32_t cand[4];
         unsigned long long key[4];
@@ -903,9 +916,11 @@ __device__ void phase2(const DevNet &N, int li, int tile, int chunk, int t) {
             if (lane == 0) {
                 D.bits[((size_t)wr * B + b) * nw + tile] = fw;
                 if (D.anyf && fw) atomicOr(D.anyf + (size_t)(t % 3) * B + b, 1u);
+                if (D.spc) nsp += __popc(fw);
             }
         }
     }
+    if (D.spc && nsp) atomicAdd(D.spc + t % 3, nsp);
 }
 
 // ---------------------------------------------------------------------------------------

@@ -62,7 +62,12 @@ class LearningRule(ABC):
             torch.squeeze if self.source.batch_size == 1 else torch.sum
         )
         self._squeeze = self.reduction is torch.squeeze
-        self._reduction_code = _reduction_code(reduction, self.source.batch_size)
+        from ..network.topology import MeanFieldConnection
+
+        # a MeanFieldConnection passes its weight_decay in the reduction slot (reference topology.py:1957); NoOp, the only
+        # rule it runs, never reduces
+        self._reduction_code = (_abi.SNN_REDUCE_SUM if isinstance(connection, MeanFieldConnection)
+                                else _reduction_code(reduction, self.source.batch_size))
         self.weight_decay = 1.0 - weight_decay if weight_decay else 1.0
 
     def update(self, **kwargs) -> None:

@@ -12,7 +12,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from .. import _abi, _backend
-from .topology import LocalConnection2D, _MaxPoolConnection
+from .topology import LocalConnection2D, MeanFieldConnection, _MaxPoolConnection, meanfield_offsets
 
 
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
@@ -100,6 +100,13 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
         conn._fill_desc(d, dt, rule)
         return
     conn._fill_desc(d, dt, rule)
+    if d.kind == _abi.SNN_CONN_MEANFIELD:   # w in its own shape, read through the per-target offset map
+        w = conn.w
+        if w.dtype != torch.float32 or not w.is_contiguous():
+            raise TypeError("connection weights must be contiguous float32")
+        off, d.mf_stride = meanfield_offsets(conn, B)
+        d.w, d.mf_off = _ptr(w), _ptr(off)
+        return
     if d.kind in (_abi.SNN_CONN_LOCAL2D, _abi.SNN_CONN_LOCAL3D):   # [cin, n, K] weights, no bias (compute never reads b)
         w = conn.w
         if w.dtype != torch.float32 or not w.is_contiguous():
@@ -377,6 +384,8 @@ def compute_single_connection(conn, s: torch.Tensor, draw: Optional[Tuple[int, i
     B = s.shape[0]
     if isinstance(conn, _MaxPoolConnection):
         return _compute_pool(conn, s)
+    if isinstance(conn, MeanFieldConnection):
+        return _compute_meanfield(conn, s)
     _backend.require_cuda(conn.w, "connection weights")
     su8 = _as_u8(s if s.dtype in (torch.bool, torch.uint8) else (s != 0)).reshape(B, -1).contiguous()
     su8 = su8.to(conn.w.device)
@@ -388,6 +397,28 @@ def compute_single_connection(conn, s: torch.Tensor, draw: Optional[Tuple[int, i
         d.draw_seed, d.draw_step, d.draw_conn = draw[0] & 0xFFFFFFFF, draw[1] & 0xFFFFFFFF, draw[2]
     _backend.conn_compute(d, conn.source.n, conn.target.n, B, su8, out)
     return out.view(B, *conn.target.shape)
+
+
+def _compute_meanfield(conn, s: torch.Tensor) -> torch.Tensor:
+    """``MeanFieldConnection.compute(s)``: ``s.float().mean() * w``, shaped like ``w`` as the reference returns it.  The
+    operator reads all of ``s`` as one sample and writes every element of ``w`` once (offsets 0 .. w.numel() - 1)."""
+    w = conn.w
+    _backend.require_cuda(w, "connection weights")
+    if w.dtype != torch.float32 or not w.is_contiguous():
+        raise TypeError("connection weights must be contiguous float32")
+    su8 = _as_u8(s if s.dtype in (torch.bool, torch.uint8) else (s != 0)).reshape(1, -1).contiguous().to(w.device)
+    n = su8.shape[1]
+    if n >= 1 << 24:
+        raise NotImplementedError(f"MeanFieldConnection.compute on {n} spikes: the float32 mean is exact below 2**24 only")
+    if n == 0 or w.numel() == 0:   # (the reference's mean of nothing is NaN)
+        return torch.full_like(w, float("nan")) if n == 0 else torch.empty_like(w)
+    d = _abi.SnnConn()
+    conn._fill_desc(d, 1.0)
+    off = torch.arange(w.numel(), dtype=torch.int32, device=w.device)
+    d.w, d.mf_off, d.mf_stride = _ptr(w), _ptr(off), 0
+    out = torch.empty(1, w.numel(), dtype=torch.float32, device=w.device)
+    _backend.conn_compute(d, n, w.numel(), 1, su8, out)
+    return out.view(w.shape)
 
 
 def _compute_pool(conn, s: torch.Tensor) -> torch.Tensor:

@@ -136,7 +136,7 @@ class Network(torch.nn.Module):
         current spikes: the sum of ``compute`` over those connections in insertion order (network.py:211-250).
         Inside a window the kernels do this themselves (the gather phase); this host form — one single-operator
         launch per connection — serves the scripted tier and callers that step a network by hand."""
-        from .topology import MulticompartmentConnection
+        from .topology import MeanFieldConnection, MulticompartmentConnection
 
         B = self.batch_size
         cur = {}
@@ -148,6 +148,8 @@ class Network(torch.nn.Module):
                 out = _plan.compute_single_connection(conn, conn.source.s, draw=(draw[0], draw[1], k))
             else:
                 out = conn.compute(conn.source.s)
+            if isinstance(conn, MeanFieldConnection):   # shaped like w: broadcast into the input as network.py:248 adds it
+                out = out.broadcast_to((B, *self.layers[tgt].shape))
             out = out.view(B, *self.layers[tgt].shape).float()
             cur[tgt] = cur[tgt] + out if tgt in cur else out
         return cur
@@ -382,7 +384,7 @@ class Network(torch.nn.Module):
                 return True
         builtin_conns = (Tp.Connection, Tp.MulticompartmentConnection, Tp.Conv2dConnection, Tp.LocalConnection, Tp.SparseConnection,
                          Tp.MaxPool2dConnection, Tp.LocalConnection2D, Tp.Conv3dConnection, Tp.Conv1dConnection,
-                         Tp.LocalConnection3D, Tp.MaxPoo3dConnection)
+                         Tp.LocalConnection3D, Tp.MaxPoo3dConnection, Tp.MeanFieldConnection)
         for conn in self.connections.values():
             if type(conn) not in builtin_conns:
                 return True

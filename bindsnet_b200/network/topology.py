@@ -1260,6 +1260,106 @@ def check_pool(conn, s_shape) -> None:
         raise TypeError(f"{name}.firing_rates must be a contiguous float32 tensor (it is updated in place)")
 
 
+class MeanFieldConnection(AbstractConnection):
+    """A summary of the whole source population as input to every target neuron (reference: topology.py:1920-2006):
+    ``compute(s)`` is ``s.float().mean() * w``.  The mean runs over all of ``[B, *source.shape]``, the batch included, so
+    every sample receives the same batch-wide mean (a sample without spikes too), scaled by ``w``.  ``w`` may have any
+    shape that broadcasts into ``[B, *target.shape]`` without growing it (0-d, ``[n]`` of the last axis, ``[1, W]``,
+    ``[C, 1]``, ``[B, *target.shape]`` per sample...); ``Network.run`` adds the result into the target's input at the
+    connection's place in the insertion order.  Inside ``Network.run`` the generic window kernel counts each source's
+    spikes with one integer per step and forms the mean from that count, bit-identical to the reference's.
+
+    As in the reference, the constructor passes ``weight_decay`` on in the ``reduction`` slot (topology.py:1957):
+    ``reduction`` holds it, ``weight_decay`` is 0.0, and a ``reduction=`` keyword raises ``TypeError``.  Without ``w`` one
+    ``torch.randn(1)[0]`` is drawn after the rule is built; a given ``w`` is clamped only when some bound is infinite.
+    Only ``learning.NoOp`` constructs (it scales ``w`` by 1.0 and never clamps, so ``w`` does not change); the STDP rules
+    and ``MSTDP`` / ``MSTDPET`` raise.  Unlike the reference, ``norm`` raises ``NotImplementedError`` at construction (the
+    reference's ``normalize()`` fails at the end of the first run), and so does a run whose ``B * source.n`` reaches
+    2**24 (where the float32 mean is no longer the exact count over ``N``).  ``masks=`` for it raise, as for every
+    connection but the dense one."""
+
+    def __init__(
+        self,
+        source: Nodes,
+        target: Nodes,
+        nu: Optional[Union[float, Sequence[float], Sequence[torch.Tensor]]] = None,
+        weight_decay: float = 0.0,
+        w_dtype: torch.dtype = torch.float32,
+        **kwargs,
+    ) -> None:
+        if w_dtype != torch.float32:
+            raise NotImplementedError("bindsnet_b200 computes in float32 only (SURVEY.md §8b)")
+        if kwargs.get("norm", None) is not None:
+            raise NotImplementedError(
+                "MeanFieldConnection does not support norm: the reference's normalize() assigns a view to the w Parameter "
+                "(TypeError), or fails to view w as [1, target.n] (RuntimeError), at the end of the first run; this raises "
+                "at construction"
+            )
+        super().__init__(source, target, nu, weight_decay, **kwargs)   # weight_decay in the reduction slot, topology.py:1957
+        w = kwargs.get("w", None)
+        if w is None:                                                    # topology.py:1959-1965
+            if (self.wmin == -np.inf).any() or (self.wmax == np.inf).any():
+                w = torch.clamp((torch.randn(1)[0] + 1) / 10, self.wmin, self.wmax)
+            else:
+                w = self.wmin + ((torch.randn(1)[0] + 1) / 10) * (self.wmax - self.wmin)
+            w = w.to(dtype=w_dtype)
+        else:                                                            # topology.py:1966-1969
+            if (self.wmin == -np.inf).any() or (self.wmax == np.inf).any():
+                w = torch.clamp(w, self.wmin, self.wmax)
+            w = self.cast_dtype_if_needed(w, w_dtype)
+        self.w = Parameter(w.detach().clone().contiguous(), requires_grad=False)
+        self._mf_offsets = None   # (key, offsets, stride) of the last plan (meanfield_offsets)
+
+    def compute(self, s: torch.Tensor) -> torch.Tensor:
+        """``s.float().mean() * w`` (topology.py:1972-1981), shaped like ``w`` (``snn_b200_conn_compute``)."""
+        from . import _plan
+
+        return _plan.compute_single_connection(self, s)
+
+    def update(self, **kwargs) -> None:
+        """topology.py:1983-1988 -> :112-139: learning.NoOp scales ``w`` by 1.0 and does not clamp (learning.py:93-104), so
+        nothing changes; a user-defined rule runs as it does on any connection.  ``masks=`` are refused by Network.run."""
+        if kwargs.get("learning", True) and self.update_rule.rule_code is None:
+            self.update_rule.update(**kwargs)
+
+    def normalize(self) -> None:
+        """``norm`` is refused at construction, so there is nothing to normalize (topology.py:1990-1999)."""
+
+    def reset_state_variables(self) -> None:
+        """No state of its own (topology.py:2001-2006)."""
+
+    def _fill_desc(self, d: "_abi.SnnConn", dt: float, rule: bool = True) -> None:
+        d.kind = _abi.SNN_CONN_MEANFIELD
+        d.rule = _abi.SNN_RULE_NOOP
+        d.weight_decay = 1.0
+
+
+def meanfield_offsets(conn, B: int, cache: bool = True):
+    """The SNN_CONN_MEANFIELD view of ``conn.w`` (this package's or the reference's MeanFieldConnection) at batch size
+    ``B``: an int32 ``[target.n]`` tensor on ``w``'s device holding the element of ``w`` each target neuron of sample 0
+    reads, and the step between samples (0 unless ``w`` has the batch axis).  Raises what the reference raises before
+    anything runs: the ``RuntimeError`` of ``inputs += mean * w`` for a ``w`` that does not broadcast into ``[B,
+    *target.shape]`` or would grow it, and ``NotImplementedError`` where ``B * source.n`` reaches 2**24.  Cached on the
+    connection per (``w`` shape, target shape, ``B``, device) unless ``cache`` is false (the reference's objects)."""
+    w = conn.w
+    full = (int(B), *(int(v) for v in conn.target.shape))
+    key = (tuple(w.shape), full, w.device)
+    cached = getattr(conn, "_mf_offsets", None) if cache else None
+    if cached is not None and cached[0] == key:
+        return cached[1], cached[2]
+    if int(B) * int(conn.source.n) >= 1 << 24:
+        raise NotImplementedError(f"MeanFieldConnection with B * source.n = {int(B) * int(conn.source.n)} spikes per step: the "
+                                  "float32 mean is exact below 2**24 only")
+    # network.py:248: inputs[target] += s.float().mean() * w, with the reference's own error for a shape that fails
+    torch.empty(full, device="meta").add_(torch.empty(tuple(w.shape), device="meta"))
+    idx = torch.arange(w.numel(), dtype=torch.int64).view(tuple(w.shape)).broadcast_to(full).reshape(full[0], -1)
+    stride = int(idx[1, 0] - idx[0, 0]) if full[0] > 1 else 0
+    off = idx[0].to(torch.int32).contiguous().to(w.device)
+    if cache:
+        conn._mf_offsets = (key, off, stride)
+    return off, stride
+
+
 def _unsupported(name: str, where: str):
     class _Unsupported:
         __doc__ = f"``{name}`` (reference: {where}) — not on the accelerated path (SURVEY.md §8f)."
@@ -1276,4 +1376,3 @@ def _unsupported(name: str, where: str):
 
 MaxPool1dConnection = _unsupported("MaxPool1dConnection", "topology.py:1028-1121")
 LocalConnection1D = _unsupported("LocalConnection1D", "topology.py:1487-1620")
-MeanFieldConnection = _unsupported("MeanFieldConnection", "topology.py:1920-2006")

@@ -165,6 +165,22 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
         d.pool_decay = _f(conn.decay)
         d.pool_rates = fr.data_ptr()
         return
+    if type(conn).__name__ == "MeanFieldConnection":
+        # topology.py:1920-2006: s.float().mean() * w, w in its own shape and read through a per-target offset map;
+        # learning.NoOp leaves it as it is (learning.py:93-104)
+        from .network.topology import meanfield_offsets
+
+        if conn.norm is not None:
+            raise NotImplementedError("MeanFieldConnection with norm: the reference's normalize() fails at the end of the run")
+        if type(conn.update_rule).__name__ != "NoOp":
+            raise NotImplementedError(f"{type(conn.update_rule).__name__} on a MeanFieldConnection")
+        w = conn.w
+        if w.dtype != torch.float32 or not w.is_contiguous():
+            raise TypeError("MeanFieldConnection.w must be contiguous float32")
+        off, d.mf_stride = meanfield_offsets(conn, int(conn.source.s.shape[0]) if B is None else int(B), cache=False)
+        keep.append(off)
+        d.kind, d.rule, d.w, d.mf_off = _abi.SNN_CONN_MEANFIELD, _abi.SNN_RULE_NOOP, w.data_ptr(), off.data_ptr()
+        return
     if type(conn).__name__ == "LocalConnection2D":
         # topology.py:1623-1767: w [in_channels, n_filters * conv_prod, kernel_prod], b never read; the geometry of the
         # reference's unfold (no padding, no dilation) and its view of the output as the target's shape

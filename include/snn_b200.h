@@ -194,6 +194,21 @@ extern "C" {
                                 SNN_CONN_MAXPOOL2D.  Generic tier only; not in a plan that also holds an SNN_CONN_SPARSE
                                 connection, MCC features or per-neuron parameters, and never into a PassThroughNodes
                                 layer; a library older than the kind refuses it with SNN_ERR_UNSUPPORTED */
+#define SNN_CONN_MEANFIELD 10 /* MeanFieldConnection: s.float().mean() * w, topology.py:1920-2006.  The mean runs over the
+                                whole [B, n_src] spike tensor, the batch included, so every sample's input depends on
+                                every sample's spikes:
+                                  mean = fl((float)count / (float)(B * n_src)),  count = the number of spikes in s
+                                  out[b, j] = fl(mean * w[mf_off[j] + b * mf_stride])
+                                (exact while B * n_src < 2^24: the reference's CPU sum of 0 / 1 floats is the integer
+                                count).  w is the connection's weight tensor in any shape that broadcasts into
+                                [B, *target.shape] without growing it; mf_off [n_tgt] (int32) is the element of w target
+                                neuron j of sample 0 reads, and mf_stride the step of a further sample (0 unless w has the
+                                batch axis).  The result is added into the target's input at the connection's place in
+                                the insertion order (network.py:244-248).  b is NULL; rule SNN_RULE_NOOP (w is never
+                                written: learning.NoOp scales it by 1.0 and does not clamp) or SNN_RULE_NONE; no normalize,
+                                no mask; the target is not a PassThroughNodes layer.  Every instantiation of the generic
+                                kernel takes it; generic tier only (a forced tier 2 or 3 is SNN_ERR_UNSUPPORTED).  A
+                                library older than the kind refuses it with SNN_ERR_UNSUPPORTED */
 #define SNN_RULE_NONE 0       /* MCC_learning.NoOp: update() does nothing    MCC_learning.py:120-146 */
 #define SNN_RULE_NOOP 1        /* learning.NoOp: weight decay only, no clamp  learning.py:107-146     */
 #define SNN_RULE_POSTPRE 2     /* learning.PostPre._connection_update         learning.py:390-420     */
@@ -355,7 +370,8 @@ typedef struct snn_conn {
        in place by SNN_RULE_NOOP.  A malformed pattern is reported as SNN_ERR_BAD_ARG (in *err_flag by the window).
        SNN_CONN_CONV3D (topology.py:847-1025) keeps its depth axis in the same storage: source depth din, target depth
        dout, kernel depth kd, stride sd, padding pd; SNN_CONN_MAXPOOL3D also its depth dilation dd (read by no other
-       kind).  A connection is never both, so the layout is the one without it. */
+       kind).  SNN_CONN_MEANFIELD keeps its offset map and per-sample stride there.  A connection is never two of these
+       kinds, so the layout is the one without them. */
     union {
         struct {
             const int32_t *sp_rowptr;
@@ -364,6 +380,10 @@ typedef struct snn_conn {
         };
         struct {
             int32_t din, dout, kd, sd, pd, dd;
+        };
+        struct {
+            const int32_t *mf_off;   /* SNN_CONN_MEANFIELD: [n_tgt] element of w per target neuron (sample 0) */
+            int32_t mf_stride;       /* SNN_CONN_MEANFIELD: elements of w between consecutive samples (0: shared) */
         };
     };
     /* SNN_CONN_MCC with Probability / Mask / Intensity features besides its Weight (topology.py:437-479).  Each is an

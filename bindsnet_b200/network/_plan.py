@@ -129,8 +129,7 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
         return
     if d.kind == _abi.SNN_CONN_SPARSE:
         fill_sparse(d, conn)
-        b = getattr(conn, "b", None)
-        d.b = _ptr(b) if b is not None else None
+        d.b = _ptr(target_bias(conn, B))
         return
     w = conn.w
     if w.dtype != torch.float32 or not w.is_contiguous():
@@ -146,11 +145,51 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
     static = d.rule == _abi.SNN_RULE_NONE or (d.rule == _abi.SNN_RULE_NOOP and d.weight_decay in (0.0, 1.0))
     if static and not d.has_norm:
         d.structure, d.structure_val = weight_structure(conn, w)
-    b = getattr(conn, "b", None)
-    d.b = _ptr(b) if b is not None else None
+    if d.kind == _abi.SNN_CONN_DENSE:
+        d.b = _ptr(target_bias(conn, B))
+    else:
+        b = getattr(conn, "b", None)
+        d.b = _ptr(b) if b is not None else None
     if d.kind == _abi.SNN_CONN_MCC:
         fill_features(d, conn)
     check_squeeze(d, conn, B)
+
+
+def target_bias(conn, B: int) -> Optional[torch.Tensor]:
+    """The bias of a dense ``Connection`` or a ``SparseConnection`` as the kernels read it: ``b[j]`` for every target
+    neuron j, contiguous float32.  The reference adds ``b`` to the ``[B, n_tgt]`` product (topology.py:342-345), so every
+    bias that broadcasts there is valid.  One that is the same for every sample (0-d, ``[1]``, ``[n_tgt]``, ``[1, n_tgt]``,
+    any strides) is read in place when it already lies contiguously, so that in-place edits take effect, and otherwise
+    through a contiguous ``[n_tgt]`` copy cached on the connection until the bias changes (the cache keeps the copy alive
+    as long as any plan that points at it)."""
+    b = getattr(conn, "b", None)
+    if b is None:
+        return None
+    name, n = type(conn).__name__, conn.target.n
+    if b.dtype != torch.float32:
+        raise TypeError(f"{name}.b must be float32, got {b.dtype}")
+    shape = tuple(b.shape)
+    try:
+        ok = torch.broadcast_shapes(shape, (B, n))[-2:] == (B, n) and all(k == 1 for k in shape[:-2])
+    except RuntimeError:
+        ok = False
+    if not ok:   # (the reference's sum, or the view of its result as [B, *target.shape], fails)
+        raise RuntimeError(f"{name}.b of shape {list(shape)} does not broadcast to the [{B}, {n}] input of its target")
+    if b.dim() >= 2 and shape[-2] != 1:
+        raise NotImplementedError(f"{name}.b of shape {list(shape)}: a per-sample bias is not implemented by the CUDA core "
+                                  f"(it adds one value per target neuron)")
+    v = b.detach()
+    while v.dim() > 2:
+        v = v[0]
+    v = v.broadcast_to((1, n)).reshape(n)   # (always a view of b)
+    if v.is_contiguous():
+        return v
+    key = (b.data_ptr(), b._version, shape, tuple(b.stride()), str(b.device))
+    cached = getattr(conn, "_b200_bias", None)
+    if cached is None or cached[0] != key:
+        cached = (key, v.contiguous(), b)   # (b stays referenced, so its address cannot be reused by another bias)
+        conn._b200_bias = cached
+    return cached[1]
 
 
 def check_squeeze(d: "_abi.SnnConn", conn, B: int) -> None:

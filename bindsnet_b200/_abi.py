@@ -18,6 +18,7 @@ SNN_CONN_DENSE, SNN_CONN_MCC, SNN_CONN_CONV2D, SNN_CONN_SPARSE, SNN_CONN_MAXPOOL
 SNN_CONN_CONV3D, SNN_CONN_CONV1D, SNN_CONN_LOCAL3D, SNN_CONN_MAXPOOL3D, SNN_CONN_MEANFIELD = 6, 7, 8, 9, 10
 SNN_RULE_NONE, SNN_RULE_NOOP, SNN_RULE_POSTPRE, SNN_RULE_WDEP_POSTPRE, SNN_RULE_MCC_POSTPRE, SNN_RULE_MSTDP, SNN_RULE_HEBBIAN = 0, 1, 2, 3, 4, 5, 6
 SNN_RULE_MSTDPET = 7
+SNN_RULE_AVG = 0x100
 SNN_REDUCE_SUM, SNN_REDUCE_MEAN = 0, 1
 SNN_EXT_NONE, SNN_EXT_U8, SNN_EXT_F32 = 0, 1, 2
 SNN_W_DENSE, SNN_W_DIAG, SNN_W_OFFDIAG = 0, 1, 2
@@ -147,8 +148,26 @@ class _FeaturesOrSynapse(C.Union):
     _fields_ = [("_feat", _FeatureFields), ("_syn", _SynapseFields)]
 
 
+class _RewardFields(C.Structure):
+    _fields_ = [("reward", C.c_float), ("a_plus", C.c_float), ("a_minus", C.c_float), ("p_plus_decay", C.c_float),
+                ("p_minus_decay", C.c_float), ("p_plus", C.c_void_p), ("p_minus", C.c_void_p), ("elig", C.c_void_p),
+                ("mst_spre", C.c_void_p), ("mst_spost", C.c_void_p)]
+
+
+class _AverageFields(C.Structure):
+    _fields_ = [("avg_pre", C.c_void_p), ("avg_post", C.c_void_p), ("avg_rows", C.c_void_p), ("avg_cols", C.c_void_p),
+                ("avg_k", C.c_int32), ("avg_idx_pre", C.c_int32), ("avg_idx_post", C.c_int32), ("avg_continues", C.c_int32)]
+
+
+class _RewardOrAverage(C.Union):
+    """The storage the reward-modulated rules' state and MCC PostPre's averaging state (SNN_RULE_AVG) share."""
+
+    _anonymous_ = ("_reward", "_avg")
+    _fields_ = [("_reward", _RewardFields), ("_avg", _AverageFields)]
+
+
 class SnnConn(C.Structure):
-    _anonymous_ = ("_u", "_f")
+    _anonymous_ = ("_r", "_u", "_f")
     _fields_ = [
         ("kind", C.c_int32),
         ("src", C.c_int32),
@@ -173,16 +192,7 @@ class SnnConn(C.Structure):
         ("cout", C.c_int32), ("hout", C.c_int32), ("wout", C.c_int32),
         ("kh", C.c_int32), ("kw", C.c_int32), ("sh", C.c_int32), ("sw", C.c_int32),
         ("ph", C.c_int32), ("pw", C.c_int32), ("dh", C.c_int32), ("dw", C.c_int32),
-        ("reward", C.c_float),
-        ("a_plus", C.c_float),
-        ("a_minus", C.c_float),
-        ("p_plus_decay", C.c_float),
-        ("p_minus_decay", C.c_float),
-        ("p_plus", C.c_void_p),
-        ("p_minus", C.c_void_p),
-        ("elig", C.c_void_p),
-        ("mst_spre", C.c_void_p),
-        ("mst_spost", C.c_void_p),
+        ("_r", _RewardOrAverage),
         ("mask", C.c_void_p),
         ("e_trace", C.c_void_p),
         ("e_trace_decay", C.c_float),

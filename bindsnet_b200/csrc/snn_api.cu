@@ -32,12 +32,33 @@ static int pn_check(const snn_layer_t &L) {
     return SNN_OK;
 }
 
+// An averaged MCC PostPre (snn_b200.h SNN_RULE_AVG): the rule and kind it extends, its state, no mask.
+static int avg_check(const snn_conn_t &C) {
+    if ((C.rule & ~SNN_RULE_AVG) != SNN_RULE_MCC_POSTPRE || C.kind != SNN_CONN_MCC || C.mask) return SNN_ERR_UNSUPPORTED;
+    if (C.avg_k < 1 || C.avg_idx_pre < 0 || C.avg_idx_pre >= C.avg_k || C.avg_idx_post < 0 || C.avg_idx_post >= C.avg_k)
+        return SNN_ERR_BAD_ARG;
+    if (!C.avg_pre || !C.avg_post || !C.avg_rows || !C.avg_cols) return SNN_ERR_BAD_ARG;
+    return SNN_OK;
+}
+
 // The plan every check and kernel below reads: the kinds without SNN_NODE_PN, pn_mask cleared on the LIF / DC layers
-// that do not carry the flag (their storage is CurrentLIFNodes' otherwise).  *pn: some layer uses a per-neuron row.
+// that do not carry the flag (their storage is CurrentLIFNodes' otherwise); the rules without SNN_RULE_AVG, avg_k
+// cleared on every other MCC PostPre (snn_is_avg).  *pn: some layer uses a per-neuron row.
 static int strip_pn(const snn_net_t *net, snn_net_t *out, bool *pn) {
     *pn = false;
     if (!net || net->n_layers < 0 || net->n_layers > SNN_MAX_LAYERS) return SNN_ERR_BAD_ARG;
+    if (net->n_conns < 0 || net->n_conns > SNN_MAX_CONNS) return SNN_ERR_BAD_ARG;
     *out = *net;
+    for (int c = 0; c < net->n_conns; ++c) {
+        snn_conn_t &C = out->conns[c];
+        if (C.rule & SNN_RULE_AVG) {
+            const int rc = avg_check(C);
+            if (rc != SNN_OK) return rc;
+            C.rule &= ~SNN_RULE_AVG;
+        } else if (C.rule == SNN_RULE_MCC_POSTPRE) {
+            C.avg_k = 0;
+        }
+    }
     for (int l = 0; l < net->n_layers; ++l) {
         snn_layer_t &L = out->layers[l];
         if (L.kind & SNN_NODE_PN) {
@@ -183,6 +204,13 @@ static bool has_feat(const snn_net_t *net) {
     return false;
 }
 
+// some MCC PostPre averages its updates (snn_b200.h SNN_RULE_AVG)
+static bool has_avg(const snn_net_t *net) {
+    for (int c = 0; c < net->n_conns; ++c)
+        if (snn_is_avg(net->conns[c])) return true;
+    return false;
+}
+
 // some dense connection carries per-synapse bounds or rates (snn_b200.h)
 static bool has_syn(const snn_net_t *net) {
     for (int c = 0; c < net->n_conns; ++c)
@@ -270,6 +298,16 @@ static size_t layout_generic(const snn_net_t *net, const snn_run_opts_t *o, char
         if (N) N->sp[c].out = (float *)(ws + off);
         off += align_up(sizeof(float) * B * nt);
     }
+    // averaged MCC PostPre: the second slot of the slot bitmaps (DevAvg)
+    for (int c = 0; c < net->n_conns; ++c) {
+        const snn_conn_t &C = net->conns[c];
+        if (!snn_is_avg(C)) continue;
+        const size_t nr = (size_t)C.avg_k * ((net->layers[C.src].n + 31) / 32), nc = (size_t)C.avg_k * ((net->layers[C.tgt].n + 31) / 32);
+        if (N) { N->avg[c].rows[0] = C.avg_rows; N->avg[c].cols[0] = C.avg_cols; N->avg[c].rows[1] = (uint32_t *)(ws + off); }
+        off += align_up(sizeof(uint32_t) * nr);
+        if (N) N->avg[c].cols[1] = (uint32_t *)(ws + off);
+        off += align_up(sizeof(uint32_t) * nc);
+    }
     // MaxPool2d / MaxPoo3dConnections: the second slot of the rates (pool_rate_slot)
     for (int c = 0; c < net->n_conns; ++c) {
         if (!snn_is_maxpool(net->conns[c].kind)) continue;
@@ -296,6 +334,11 @@ static int select_tier(const snn_net_t *net, const snn_run_opts_t *opts, bool pn
     // snn_pool_inst_kind names, and SubtractiveResetIFNodes or PassThroughNodes), not combinations (and one for plans
     // with per-synapse bounds or rates)
     if ((int)has_sparse(net) + (int)has_feat(net) + (int)has_pool(net) + (int)has_syn(net) > 1) return 0;
+    // averaged MCC PostPre: two more instantiations, alone or with features; generic tier only
+    if (has_avg(net)) {
+        if (pn || has_sparse(net) || has_pool(net) || has_syn(net)) return 0;
+        return (opts->tier == 0 || opts->tier == 1) && !opts->delta_w && !opts->delta_theta ? 1 : 0;
+    }
     // per-neuron parameters: two more instantiations, alone or with per-synapse tensors; the fused kernels read scalars
     if (pn) {
         if (has_sparse(net) || has_feat(net) || has_pool(net)) return 0;
@@ -331,7 +374,7 @@ size_t snn_b200_workspace_bytes(const snn_net_t *net0, const snn_run_opts_t *opt
     const snn_net_t *net = &P;
     if (validate(net, opts) != SNN_OK) return 0;
     size_t g = layout_generic(net, opts, nullptr, nullptr);
-    if (pn || has_sparse(net) || has_feat(net) || has_pool(net) || has_syn(net) || has_meanfield(net)) return g;
+    if (pn || has_sparse(net) || has_feat(net) || has_pool(net) || has_syn(net) || has_meanfield(net) || has_avg(net)) return g;
     size_t f = snn_fused_dc_supported(net, opts) ? snn_fused_dc_workspace_bytes(net, opts) : 0;
     size_t f2 = snn_fused_dc2_supported(net, opts) ? snn_fused_dc2_workspace_bytes(net, opts) : 0;
     if (f2 > f) f = f2;
@@ -376,6 +419,7 @@ int snn_b200_run_window(const snn_net_t *net0, const snn_run_opts_t *opts, void 
         if (C.kind == SNN_CONN_MCC && (C.f_prob || C.f_mask || C.f_int)) N.any_feat = 1;
     }
     N.any_pool = has_pool(net) ? 1 : 0;
+    N.any_avg = has_avg(net) ? 1 : 0;
     if (cudaMemsetAsync(N.bar, 0, sizeof(unsigned int) * SNN_BAR_ZERO_WORDS, stream) != cudaSuccess) return SNN_ERR_CUDA;
     const int e = snn_generic_launch(N, stream);
     if (e != 0) {

@@ -87,6 +87,16 @@ __host__ __device__ inline int sparse_block_width(int n_src, int n_tgt, int B, i
     return bw;
 }
 
+// The slot bitmaps of an averaged MCC PostPre (snn_b200.h SNN_RULE_AVG), double-buffered like DevMstdp: step t reads slot
+// (t + T) & 1 and writes the other one, slot 0 is the caller's avg_rows / avg_cols, slot 1 lives in the workspace.  Every
+// unit of the learning phase reads a slot's previous bitmap while the one that owns its word writes the new one.
+struct DevAvg {
+    uint32_t *rows[2], *cols[2];
+};
+// The plan (after snn_api.cu's strip) runs a connection's MCC PostPre with averaging: the library clears avg_k on every
+// other MCC PostPre connection, and no other rule reads the field.
+__host__ __device__ __forceinline__ bool snn_is_avg(const snn_conn_t &C) { return C.rule == SNN_RULE_MCC_POSTPRE && C.avg_k > 0; }
+
 struct DevNet {
     int32_t n_layers, n_conns, learning, T, B, normalize, total_items, any_one_spike;
     int32_t any_mask;             // some connection carries a mask (Network.run(..., masks=...))
@@ -107,6 +117,8 @@ struct DevNet {
     int32_t any_pool;             // some connection is of a kind snn_pool_inst_kind names, or some layer is an
                                   // SNN_NODE_SUBIF / SNN_NODE_PASSTHROUGH one: the plan runs the POOL instantiation
     float *pool_r1[SNN_MAX_CONNS];   // MaxPool2d / MaxPoo3dConnection: the workspace slot of its rates (pool_rate_slot)
+    DevAvg avg[SNN_MAX_CONNS];    // MCC PostPre with averaging (snn_is_avg)
+    int32_t any_avg;              // some connection is one: the plan runs an AVG instantiation
 };
 
 // A MaxPool2dConnection's or MaxPoo3dConnection's rates, double-buffered: the gather of step t reads slot

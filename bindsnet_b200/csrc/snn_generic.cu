@@ -65,7 +65,9 @@ __device__ __forceinline__ void sparse_unit(const DevNet &N, int u, int &c, int 
 // plans without them run the instantiation whose code never reads those fields.  Not combined with SPARSE, FEAT or POOL.
 // PN: some LIF / DC layer carries per-neuron parameters (snn_b200.h SNN_NODE_PN); phases 1 and 2 and the theta of the
 // last step read a lane's own values where the other instantiations read the layer's scalars.  Combined with SYN only.
-template <int CTAS, bool SPARSE, bool FEAT, bool POOL, bool SYN = false, bool PN = false>
+// AVG: some MCC PostPre averages its updates (snn_b200.h SNN_RULE_AVG); only the learning phase (and the prologue's copy
+// of the slot bitmaps) differs.  Combined with FEAT only.
+template <int CTAS, bool SPARSE, bool FEAT, bool POOL, bool SYN = false, bool PN = false, bool AVG = false>
 __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(const __grid_constant__ DevNet N) {
 #ifdef SNN_EMU
     float *smem = emu::tls_cta->dyn_smem;
@@ -114,6 +116,15 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                     const size_t ne = Bz * (size_t)C.cout * C.cin * C.kh * C.kw;
                     for (size_t k = start; k < ne; k += stride) Ms.el[1][k] = Ms.el[0][k];
                 }
+            }
+        // the slot bitmaps of an averaged MCC PostPre, by the same rule (DevAvg)
+        if (AVG && N.learning && (N.T & 1) && tile == 0)
+            for (int c = 0; c < N.n_conns; ++c) {
+                const snn_conn_t &C = N.conns[c];
+                if (C.tgt != li || !snn_is_avg(C)) continue;
+                const size_t nr = (size_t)C.avg_k * N.layers[C.src].nw, nc = (size_t)C.avg_k * D.nw;
+                for (size_t k = threadIdx.x; k < nr; k += SNN_GEN_THREADS) N.avg[c].rows[1][k] = N.avg[c].rows[0][k];
+                for (size_t k = threadIdx.x; k < nc; k += SNN_GEN_THREADS) N.avg[c].cols[1][k] = N.avg[c].cols[0][k];
             }
         // MaxPool2d / MaxPoo3dConnection rates of step 0: the caller's rates advanced by the incoming spikes s(-1); in
         // one-step mode with the source earlier in the insertion order step 0 advances them itself, from slot
@@ -199,7 +210,9 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                 } else {
                     const int rcn = N.p3_rc[c], tile = v / rcn, rc = v - tile * rcn;
                     const int nwS = N.layers[C.src].nw;
-                    phase3<SYN>(N, c, tile, (int)((long long)rc * nwS / rcn), (int)((long long)(rc + 1) * nwS / rcn), t, M);
+                    const int wg0 = (int)((long long)rc * nwS / rcn), wg1 = (int)((long long)(rc + 1) * nwS / rcn);
+                    if (AVG && snn_is_avg(C)) phase3_mcc_avg(N, c, tile, wg0, wg1, t, M);
+                    else phase3<SYN>(N, c, tile, wg0, wg1, t, M);
                 }
             }
             GPROF(4)
@@ -330,7 +343,11 @@ int snn_generic_launch(DevNet &N, cudaStream_t) {
     int sms = 3;
     if (const char *v = getenv("SNN_EMU_SMS")) sms = atoi(v) > 0 ? atoi(v) : 3;
     const int grid = plan_units(N, sms * 2);
-    if (N.sp_units) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, true, false, false>(*(const DevNet *)a); }, &N);
+    if (N.any_avg && N.any_feat)
+        emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, true, false, false, false, true>(*(const DevNet *)a); }, &N);
+    else if (N.any_avg)
+        emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, false, false, false, true>(*(const DevNet *)a); }, &N);
+    else if (N.sp_units) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, true, false, false>(*(const DevNet *)a); }, &N);
     else if (N.any_feat) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, true, false>(*(const DevNet *)a); }, &N);
     else if (N.any_pool) emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, true>(*(const DevNet *)a); }, &N);
     else if (snn_dev_has_pn(N) && std::any_of(N.conns, N.conns + N.n_conns, snn_has_syn))
@@ -357,8 +374,10 @@ int snn_generic_launch(DevNet &N, cudaStream_t stream) {
     const bool syn = std::any_of(N.conns, N.conns + N.n_conns, snn_has_syn);
     const bool pn = snn_dev_has_pn(N);
     bool three = false;
-    if (const char *v = getenv("SNN_B200_GVAR")) three = !sparse && !N.any_feat && !N.any_pool && !syn && !pn && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
-    const void *kern = three ? (const void *)snn_generic_window<3, false, false, false>
+    if (const char *v = getenv("SNN_B200_GVAR")) three = !sparse && !N.any_feat && !N.any_pool && !syn && !pn && !N.any_avg && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
+    const void *kern = N.any_avg ? (N.any_feat ? (const void *)snn_generic_window<2, false, true, false, false, false, true>
+                                               : (const void *)snn_generic_window<2, false, false, false, false, false, true>)
+                     : three ? (const void *)snn_generic_window<3, false, false, false>
                      : sparse ? (const void *)snn_generic_window<2, true, false, false>
                      : pn ? (syn ? (const void *)snn_generic_window<2, false, false, false, true, true>
                                : (const void *)snn_generic_window<2, false, false, false, false, true>)

@@ -273,6 +273,17 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS) conn_update_kernel(const __gr
     phase3<SYN>(N, ci, blockIdx.x, 0, N.layers[N.conns[ci].src].nw, 0, M);
 }
 
+// The single-operator update of an averaged MCC PostPre (snn_b200.h SNN_RULE_AVG): one step of the window's learning
+// phase, a CTA per column tile; the slot bitmaps are read from a copy (DevAvg slot 1) and written to the caller's.
+__global__ void __launch_bounds__(SNN_GEN_THREADS) avg_update_kernel(const __grid_constant__ DevNet N, int ci) {
+    SNN_DYN_SHARED(float, smem);
+    const GenSmem M = gen_carve(smem, N.B);
+    phase3_mcc_avg(N, ci, blockIdx.x, 0, N.layers[N.conns[ci].src].nw, 0, M);
+}
+__global__ void copy_u32_kernel(uint32_t *dst, const uint32_t *src, size_t n) {
+    for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (size_t)gridDim.x * blockDim.x) dst[k] = src[k];
+}
+
 __global__ void __launch_bounds__(SNN_GEN_THREADS) conn_normalize_kernel(snn_conn_t C, int ns, int nt) {
     SNN_SHARED(float, s_part, (SNN_NORM_CHUNKS + 1) * 32);
     normalize_tile(C, ns, nt, blockIdx.x, s_part);
@@ -429,7 +440,15 @@ int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, 
 
 int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *workspace, size_t workspace_bytes, void *stream_) {
     if (!net || ci < 0 || ci >= net->n_conns || B <= 0 || !workspace) return SNN_ERR_BAD_ARG;
-    const snn_conn_t &C = net->conns[ci];
+    snn_conn_t C = net->conns[ci];
+    const bool avg = (C.rule & SNN_RULE_AVG) != 0;
+    if (avg) {   // MCC PostPre with averaging (snn_b200.h): the plain rule's checks below, then its own kernel
+        if (C.kind != SNN_CONN_MCC || (C.rule & ~SNN_RULE_AVG) != SNN_RULE_MCC_POSTPRE || C.mask) return SNN_ERR_UNSUPPORTED;
+        if (C.avg_k < 1 || C.avg_idx_pre < 0 || C.avg_idx_pre >= C.avg_k || C.avg_idx_post < 0 || C.avg_idx_post >= C.avg_k ||
+            !C.avg_pre || !C.avg_post || !C.avg_rows || !C.avg_cols)
+            return SNN_ERR_BAD_ARG;
+        C.rule = SNN_RULE_MCC_POSTPRE;
+    }
     if (C.src < 0 || C.src >= net->n_layers || C.tgt < 0 || C.tgt >= net->n_layers) return SNN_ERR_BAD_ARG;
     if (C.kind == SNN_CONN_SPARSE) {   // learning.NoOp: the stored values decay (learning.py:93-94); no other rule on a fixed pattern
         if (C.rule != SNN_RULE_NONE && C.rule != SNN_RULE_NOOP) return SNN_ERR_UNSUPPORTED;
@@ -486,6 +505,7 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
     memset(&N, 0, sizeof(N));
     N.n_layers = net->n_layers; N.n_conns = net->n_conns; N.learning = 1; N.T = 1; N.B = B;
     for (int c = 0; c < net->n_conns; ++c) N.conns[c] = net->conns[c];
+    N.conns[ci] = C;
     size_t off = 0;
     const int ends[2] = {C.src, C.tgt};
     for (int e = 0; e < 2; ++e) {
@@ -521,6 +541,21 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
         return cuda_rc(cudaGetLastError());
     }
     const size_t smem = gen_smem_bytes(B);
+    if (avg) {   // the bitmaps this step reads: a copy of the caller's (the kernel rewrites them while other CTAs read)
+        const size_t nr = (size_t)C.avg_k * N.layers[C.src].nw, nc = (size_t)C.avg_k * N.layers[C.tgt].nw;
+        DevAvg &A = N.avg[ci];
+        A.rows[0] = C.avg_rows; A.cols[0] = C.avg_cols;
+        A.rows[1] = (uint32_t *)((char *)workspace + off);
+        off += (sizeof(uint32_t) * nr + 255) / 256 * 256;
+        A.cols[1] = (uint32_t *)((char *)workspace + off);
+        off += (sizeof(uint32_t) * nc + 255) / 256 * 256;
+        if (off > workspace_bytes) return SNN_ERR_WORKSPACE;
+        SNN_LAUNCH(copy_u32_kernel, 1, 256, 0, stream, A.rows[1], (const uint32_t *)C.avg_rows, nr);
+        SNN_LAUNCH(copy_u32_kernel, 1, 256, 0, stream, A.cols[1], (const uint32_t *)C.avg_cols, nc);
+        cudaFuncSetAttribute(avg_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        SNN_LAUNCH(avg_update_kernel, N.layers[C.tgt].nw, SNN_GEN_THREADS, smem, stream, N, ci);
+        return cuda_rc(cudaGetLastError());
+    }
     if (syn) {
         cudaFuncSetAttribute(conn_update_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         SNN_LAUNCH(conn_update_kernel<true>, N.layers[C.tgt].nw, SNN_GEN_THREADS, smem, stream, N, ci);

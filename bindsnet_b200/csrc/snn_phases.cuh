@@ -1181,6 +1181,178 @@ __device__ void phase3(const DevNet &N, int ci, int tile, int wg0, int wg1, int 
 }
 
 // ---------------------------------------------------------------------------------------
+// phase 3 for MCC_learning.PostPre with average_update (MCC_learning.py:210-302; snn_b200.h SNN_RULE_AVG).  Same units
+// as phase3 (connection, 32-column tile, chunk of source row groups), a warp per row group, a lane per column.  A pre
+// slot is zero outside the rows that had a spike in its step and a post slot outside the columns, so the slot bitmaps
+// bound every pass: a slot write touches the rows (columns) active now and those of the slot's previous occupant (set to
+// zero); the mean of an element sums, in ascending slot order from +0, only the slots whose bitmap covers it (the others
+// hold zeros, which leave such a sum as it is); an element no slot covers is left alone.  With large batches nearly
+// every row is active and the passes are dense.  Order per element: pre slot, pre mean, post slot, post mean, decay,
+// clamp.  The shared accumulators of a warp hold first U (the step's pre-synaptic term), then the pre sums, then V,
+// then the post sums.
+__device__ void phase3_mcc_avg(const DevNet &N, int ci, int tile, int wg0, int wg1, int t, const GenSmem &M) {
+    const snn_conn_t &C = N.conns[ci];
+    const DevAvg &A = N.avg[ci];
+    const DevLayer &S = N.layers[C.src], &G = N.layers[C.tgt];
+    const int B = N.B, ns = S.L.n, nt = G.L.n, nwS = S.nw, nwG = G.nw, K = C.avg_k;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int j = tile * SNN_TILE + lane;
+    const bool valid = j < nt;
+    const int wr = t & 1, in = (t + N.T) & 1, out = in ^ 1;
+    const bool pre_on = C.nu0 != 0.0f, post_on = C.nu1 != 0.0f;
+    const bool decay_on = C.weight_decay != 0.0f && C.weight_decay != 1.0f;
+    const bool full = decay_on || (C.has_clamp && t == 0);
+    const bool mean = C.reduction == SNN_REDUCE_MEAN;
+    const float Bf = (float)B, Kf = (float)K;
+    const int pp = (C.avg_idx_pre + t) % K, pq = (C.avg_idx_post + t) % K;   // the slots this step writes
+    const bool apply_pre = pre_on && (C.avg_continues || (pp + 1) % K == 0);
+    const bool apply_post = post_on && (C.avg_continues || (pq + 1) % K == 0);
+    const size_t KS = (size_t)ns * nt;
+    const uint32_t *rows_in = A.rows[in], *cols_in = A.cols[in];
+
+    // the columns of this tile with a post-synaptic spike now, and those any post slot covers after this step
+    // the target traces of the tile times nu0, [B][32], when they fit (read by every row group)
+    if (pre_on && M.xt) {
+        for (int b = warp; b < B; b += SNN_GEN_WARPS) M.xt[b * 32 + lane] = valid ? __ldcg(G.L.x + (size_t)b * nt + j) * C.nu0 : 0.0f;
+        __syncthreads();
+    }
+    uint32_t cnow = 0, cunion = 0, cold = 0;
+    if (post_on) {
+        for (int b = lane; b < B; b += 32) cnow |= __ldcg(G.bits + ((size_t)wr * B + b) * nwG + tile);
+        #pragma unroll
+        for (int o = 16; o > 0; o >>= 1) cnow |= __shfl_xor_sync(0xffffffffu, cnow, o);
+        for (int q = 0; q < K; ++q) {
+            const uint32_t c = q == pq ? cnow : __ldcg(cols_in + (size_t)q * nwG + tile);
+            cunion |= c;
+            if (wg0 == 0 && warp == 0 && lane == 0) A.cols[out][(size_t)q * nwG + tile] = c;
+        }
+        cold = __ldcg(cols_in + (size_t)pq * nwG + tile);
+    }
+    float *acc = M.acc + warp * (32 * 32);
+    for (int wg = wg0 + warp; wg < wg1; wg += SNN_GEN_WARPS) {
+        const int i0 = wg * 32;
+        const int nr = min(32, ns - i0);
+        uint32_t pre_applied = 0;
+        if (pre_on) {
+            // U of the rows active now: the samples ascending from +0
+            for (int r = 0; r < 32; ++r) acc[r * 32 + lane] = 0.0f;
+            __syncwarp();
+            uint32_t rnow = 0;
+            for (int b0 = 0; b0 < B; b0 += 32) {   // a lane per sample fetches the words, the warp walks the non-zero ones
+                const uint32_t mw = b0 + lane < B ? __ldcg(S.bits + ((size_t)wr * B + b0 + lane) * nwS + wg) : 0u;
+                for (uint32_t nz = __ballot_sync(0xffffffffu, mw != 0u); nz; nz &= nz - 1) {
+                    const int b = b0 + __ffs(nz) - 1;
+                    uint32_t word = __shfl_sync(0xffffffffu, mw, __ffs(nz) - 1);
+                    rnow |= word;
+                    const float tx = M.xt ? M.xt[b * 32 + lane] : (valid ? __ldcg(G.L.x + (size_t)b * nt + j) * C.nu0 : 0.0f);
+                    while (word) {
+                        const int r = __ffs(word) - 1;
+                        word &= word - 1;
+                        acc[r * 32 + lane] = acc[r * 32 + lane] + tx;
+                    }
+                }
+            }
+            const uint32_t rold = __ldcg(rows_in + (size_t)pp * nwS + wg);
+            float *slot = C.avg_pre + (size_t)pp * KS;
+            for (uint32_t m = rnow | rold; m; m &= m - 1) {
+                const int r = __ffs(m) - 1;
+                float u = 0.0f;
+                if ((rnow >> r) & 1u) {
+                    u = acc[r * 32 + lane];
+                    if (mean) u = u / Bf;
+                }
+                if (valid) slot[(size_t)(i0 + r) * nt + j] = u;
+            }
+            uint32_t runion = 0;
+            for (int q = 0; q < K; ++q) {
+                const uint32_t rq = q == pp ? rnow : __ldcg(rows_in + (size_t)q * nwS + wg);
+                runion |= rq;
+                if (tile == 0 && lane == 0) A.rows[out][(size_t)q * nwS + wg] = rq;
+            }
+            if (apply_pre && runion) {
+                __syncwarp();
+                for (uint32_t m = runion; m; m &= m - 1) acc[(__ffs(m) - 1) * 32 + lane] = 0.0f;
+                for (int q = 0; q < K; ++q) {
+                    const uint32_t rq = q == pp ? rnow : __ldcg(rows_in + (size_t)q * nwS + wg);
+                    const float *sq = C.avg_pre + (size_t)q * KS + (size_t)i0 * nt + j;
+                    for (uint32_t m = rq; m; m &= m - 1) {
+                        const int r = __ffs(m) - 1;
+                        if (valid) acc[r * 32 + lane] = acc[r * 32 + lane] + __ldcg(sq + (size_t)r * nt);
+                    }
+                }
+                for (uint32_t m = runion; m; m &= m - 1) {
+                    const int r = __ffs(m) - 1;
+                    float d = acc[r * 32 + lane] / Kf;
+                    d = d * C.dt_scale;
+                    float *wp = C.w + (size_t)(i0 + r) * nt + j;
+                    if (valid) *wp = __ldcg(wp) - d;
+                }
+                pre_applied = runion;
+            }
+            __syncwarp();
+        }
+        const bool col_applied = apply_post && ((cunion >> lane) & 1u);
+        if (post_on && (cnow | cold)) {
+            // V of the columns active now: the samples ascending from +0, a lane per column, the row's trace broadcast
+            for (int r = 0; r < 32; ++r) acc[r * 32 + lane] = 0.0f;
+            __syncwarp();
+            for (int b0 = 0; b0 < B; b0 += 32) {
+                const uint32_t mw = b0 + lane < B ? __ldcg(G.bits + ((size_t)wr * B + b0 + lane) * nwG + tile) : 0u;
+                for (uint32_t nz = __ballot_sync(0xffffffffu, mw != 0u); nz; nz &= nz - 1) {
+                    const int b = b0 + __ffs(nz) - 1;
+                    const uint32_t cw = __shfl_sync(0xffffffffu, mw, __ffs(nz) - 1);
+                    const float xs = lane < nr ? __ldcg(S.xpub + ((size_t)wr * B + b) * ns + i0 + lane) : 0.0f;
+                    const bool mine = (cw >> lane) & 1u;
+                    for (int r = 0; r < nr; ++r) {
+                        const float xr = __shfl_sync(0xffffffffu, xs, r);
+                        if (mine) acc[r * 32 + lane] = acc[r * 32 + lane] + xr * C.nu1;
+                    }
+                }
+            }
+            if (valid && (((cnow | cold) >> lane) & 1u)) {
+                float *slot = C.avg_post + (size_t)pq * KS + (size_t)i0 * nt + j;
+                const bool now = (cnow >> lane) & 1u;
+                for (int r = 0; r < nr; ++r) {
+                    float v = 0.0f;
+                    if (now) {
+                        v = acc[r * 32 + lane];
+                        if (mean) v = v / Bf;
+                    }
+                    slot[(size_t)r * nt] = v;
+                }
+            }
+            __syncwarp();
+        }
+        if (col_applied) {
+            for (int r = 0; r < 32; ++r) acc[r * 32 + lane] = 0.0f;
+            for (int q = 0; q < K; ++q) {
+                const uint32_t cq = q == pq ? cnow : __ldcg(cols_in + (size_t)q * nwG + tile);
+                if (!((cq >> lane) & 1u)) continue;
+                const float *sq = C.avg_post + (size_t)q * KS + (size_t)i0 * nt + j;
+                for (int r = 0; r < nr; ++r) acc[r * 32 + lane] = acc[r * 32 + lane] + __ldcg(sq + (size_t)r * nt);
+            }
+        }
+        // post mean, decay and clamp of every element a term reached (all of them in a full pass)
+        if (valid && (full || col_applied || pre_applied))
+            for (int r = 0; r < nr; ++r) {
+                if (!(full || col_applied || ((pre_applied >> r) & 1u))) continue;
+                float *wp = C.w + (size_t)(i0 + r) * nt + j;
+                float w = __ldcg(wp);
+                if (col_applied) {
+                    float d = acc[r * 32 + lane] / Kf;
+                    d = d * C.dt_scale;
+                    w = w + d;
+                }
+                if (C.weight_decay != 0.0f) w = w * C.weight_decay;
+                if (C.has_clamp) w = clampf(w, C.wmin, C.wmax);
+                *wp = w;
+            }
+        __syncwarp();
+    }
+    __syncthreads();   // the staged traces belong to the CTA's next unit
+}
+
+// ---------------------------------------------------------------------------------------
 // phase 3 for reward-modulated STDP and for convolutional connections.  The rule's state is double
 // buffered (DevMstdp): everything is READ from slot `in` and WRITTEN to slot `out`, so no thread
 // overwrites a value another thread still needs in this step.

@@ -49,6 +49,9 @@ class ShardedWindowRunner:
             if hasattr(conn, "pipeline"):  # MulticompartmentConnection[Weight]: plain-sum normalize, dt-scaled rule
                 d = _abi.SnnConn()
                 conn._fill_desc(d, float(self.network.dt))
+                if d.rule & _abi.SNN_RULE_AVG:
+                    raise NotImplementedError("PostPre(average_update>0) is not supported by ShardedWindowRunner: each rank "
+                                              "would average its own shard's updates, and the buffers would diverge")
             else:
                 rule = getattr(conn, "update_rule", None)
                 code = getattr(rule, "rule_code", None)

@@ -111,7 +111,15 @@ class NoOp(MCC_LearningRule):
 
 class PostPre(MCC_LearningRule):
     """Pair-based STDP on a ``Weight`` feature (reference: MCC_learning.py:149-302): both
-    terms are scaled by ``connection.dt`` (:262,:298), then decay and clamp (:86-110)."""
+    terms are scaled by ``connection.dt`` (:262,:298), then decay and clamp (:86-110).
+
+    ``average_update=k > 0`` (:210-220, :244-291) keeps the last k terms of each side in ``average_buffer_pre`` /
+    ``average_buffer_post`` (``[k, *w.shape]``, on the weight's device) and applies their mean times ``dt``: every update
+    with ``continues_update=True``, else on every k-th update (when the side's index wraps to 0).  A side whose rate is 0
+    never touches its buffer or index.  The buffers and ``average_buffer_index_pre`` / ``_post`` survive
+    ``reset_state_variables`` (it does nothing, :304-305); a window advances each used index by its learning steps.
+    Besides the buffers the rule keeps, per slot, the rows (pre) and columns (post) that may hold non-zero values: a slot
+    outside them is zero, which lets the kernel skip it (include/snn_b200.h SNN_RULE_AVG)."""
 
     rule_code = _abi.SNN_RULE_MCC_POSTPRE
 
@@ -141,8 +149,59 @@ class PostPre(MCC_LearningRule):
             raise NotImplementedError("This learning rule is not supported for this Connection type.")
         if enforce_polarity:
             raise NotImplementedError("enforce_polarity is not implemented by the CUDA core")
-        if kwargs.get("average_update", 0):
-            raise NotImplementedError("PostPre(average_update>0) is not implemented by the CUDA core")
+        self.average_update = kwargs.get("average_update", 0)
+        self.continues_update = kwargs.get("continues_update", False)
+        if self.average_update > 0:
+            if getattr(connection, "sparse", False) or self.feature_value.is_sparse:
+                raise NotImplementedError("PostPre(average_update>0) on sparse weights is not implemented by the CUDA core")
+            k, dev = int(self.average_update), self.feature_value.device
+            self.average_buffer_pre = torch.zeros(k, *self.feature_value.shape, device=dev)
+            self.average_buffer_post = torch.zeros_like(self.average_buffer_pre)
+            self.average_buffer_index_pre = 0
+            self.average_buffer_index_post = 0
+            n_src, n_tgt = self.source.n, self.target.n
+            self._avg_rows = torch.zeros(k, (n_src + 31) // 32, dtype=torch.int32, device=dev)
+            self._avg_cols = torch.zeros(k, (n_tgt + 31) // 32, dtype=torch.int32, device=dev)
+
+    def _prepare(self, B: int, dev: torch.device, run_kwargs: dict) -> None:
+        """The averaging state on the weight's device (moved with its contents when the network moved)."""
+        if self.average_update > 0:
+            for name in ("average_buffer_pre", "average_buffer_post", "_avg_rows", "_avg_cols"):
+                t = getattr(self, name)
+                if t.device != dev or not t.is_contiguous():
+                    setattr(self, name, t.to(dev).contiguous())
+            shape = (int(self.average_update), *self.feature_value.shape)
+            for name in ("average_buffer_pre", "average_buffer_post"):
+                t = getattr(self, name)
+                if tuple(t.shape) != shape or t.dtype != torch.float32:
+                    raise ValueError(f"PostPre.{name} must be a float32 tensor of shape {list(shape)}, got {t.dtype} {list(t.shape)}")
+
+    def _fill_desc(self, d: "_abi.SnnConn") -> None:
+        super()._fill_desc(d)
+        if self.average_update > 0:
+            d.rule = self.rule_code | _abi.SNN_RULE_AVG
+            d.avg_k = int(self.average_update)
+            d.avg_idx_pre, d.avg_idx_post = int(self.average_buffer_index_pre), int(self.average_buffer_index_post)
+            d.avg_continues = int(bool(self.continues_update))
+            d.avg_pre, d.avg_post = self.average_buffer_pre.data_ptr(), self.average_buffer_post.data_ptr()
+            d.avg_rows, d.avg_cols = self._avg_rows.data_ptr(), self._avg_cols.data_ptr()
+
+    def _advance(self, steps: int) -> None:
+        """After ``steps`` learning updates: each side whose rate is non-zero moves its index (MCC_learning.py:252-254,
+        :286-288)."""
+        if self.average_update > 0 and steps > 0:
+            k = int(self.average_update)
+            if float(self.nu[0]) != 0.0:
+                self.average_buffer_index_pre = (self.average_buffer_index_pre + steps) % k
+            if float(self.nu[1]) != 0.0:
+                self.average_buffer_index_post = (self.average_buffer_index_post + steps) % k
+
+    def update(self, **kwargs) -> None:
+        super().update(**kwargs)
+        self._advance(1)
+
+    def reset_state_variables(self) -> None:
+        """MCC_learning.py:304-305: nothing (the averaging buffers and indices persist)."""
 
 
 class _RewardModulated:

@@ -306,6 +306,7 @@ class Network(torch.nn.Module):
         if delta is not None:   # multi-GPU window: weight / theta changes go to the caller's all-reduce buffer (include/snn_b200.h)
             opts.delta_w, opts.delta_theta = delta[0].data_ptr(), delta[1].data_ptr()
         self._launch(net, opts, dev)
+        self._advance_rules(T)
         del keep
 
         for mname, lname in fused.items():
@@ -335,6 +336,16 @@ class Network(torch.nn.Module):
             self._forget_structure()
             raise
 
+    def _advance_rules(self, T: int) -> None:
+        """After a window of T steps: an averaged MCC PostPre's slot indices move by the window's updates
+        (MCC_learning.py:252-288); a window with learning off leaves them."""
+        if self.learning:
+            for conn in self.connections.values():
+                if hasattr(conn, "pipeline") and not conn.manual_update:
+                    advance = getattr(conn._weight().learning_rule, "_advance", None)
+                    if advance is not None:
+                        advance(T)
+
     def _forget_structure(self) -> None:
         """Drop the cached structure hints of the static weight matrices (``_plan.weight_structure``): after a
         device-side error they are re-verified on the next window."""
@@ -358,6 +369,7 @@ class Network(torch.nn.Module):
             opts.seed, opts.step_offset = seed & 0xFFFFFFFF, step_offset + t
             opts.one_step = int(getattr(self, "_one_step", False))
             self._launch(net, opts, self._device())
+            self._advance_rules(1)
             for m in self.monitors.values():
                 if isinstance(m, SpikeCounter) and t == 0:
                     m._begin_window(B, self._device())

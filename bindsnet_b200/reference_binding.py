@@ -331,6 +331,8 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
             d.wmin = _f(lo) if lo is not None else -math.inf
             d.wmax = _f(hi) if hi is not None else math.inf
             d.has_clamp = int(lo is not None or hi is not None)                           # MCC_learning.py:101-110
+            if getattr(rule, "average_update", 0) > 0:                                    # MCC_learning.py:210-220
+                _fill_average(d, rule, keep)
         else:
             raise NotImplementedError(f"MCC learning rule {name}")
     else:
@@ -467,6 +469,47 @@ def build_net(network, inputs: Dict[str, torch.Tensor], T: int, B: int):
     return net, keep
 
 
+def _fill_average(d: "_abi.SnnConn", rule, keep: List[torch.Tensor]) -> None:
+    """PostPre's averaging state (include/snn_b200.h SNN_RULE_AVG): the reference's buffers and indices in place, and the
+    slot bitmaps the core keeps beside them, built from the buffers (a row / column of a slot is marked when it holds a
+    non-zero value; the other slots' values are zeros)."""
+    k = int(rule.average_update)
+    pre, post = rule.average_buffer_pre, rule.average_buffer_post
+    for t in (pre, post):
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise TypeError("the averaging buffers must be contiguous float32")
+
+    def words(nz: torch.Tensor) -> torch.Tensor:   # [k, n] bool -> [k, ceil(n / 32)] int32 bit words
+        n = nz.shape[1]
+        pad = torch.zeros(k, (n + 31) // 32 * 32, dtype=torch.int64, device=nz.device)
+        pad[:, :n] = nz.to(torch.int64)
+        w = (pad.view(k, -1, 32) << torch.arange(32, device=nz.device)).sum(2)
+        return torch.where(w >= 2**31, w - 2**32, w).to(torch.int32).contiguous()
+
+    rows, cols = words((pre != 0).any(2)), words((post != 0).any(1))
+    keep += [rows, cols]
+    d.rule |= _abi.SNN_RULE_AVG
+    d.avg_k, d.avg_continues = k, int(bool(rule.continues_update))
+    d.avg_idx_pre, d.avg_idx_post = int(rule.average_buffer_index_pre), int(rule.average_buffer_index_post)
+    d.avg_pre, d.avg_post, d.avg_rows, d.avg_cols = pre.data_ptr(), post.data_ptr(), rows.data_ptr(), cols.data_ptr()
+
+
+def _advance_averages(network, T: int) -> None:
+    """After a window: each averaged PostPre's indices move by the window's updates on the sides whose rate is non-zero
+    (MCC_learning.py:252-254, :286-288)."""
+    if not network.learning:
+        return
+    for conn in network.connections.values():
+        for f in getattr(conn, "pipeline", ()):
+            rule = getattr(f, "learning_rule", None)
+            if type(rule).__name__ == "PostPre" and getattr(rule, "average_update", 0) > 0 and not conn.manual_update:
+                k = int(rule.average_update)
+                if rule.nu[0]:
+                    rule.average_buffer_index_pre = (rule.average_buffer_index_pre + T) % k
+                if rule.nu[1]:
+                    rule.average_buffer_index_post = (rule.average_buffer_index_post + T) % k
+
+
 def run_window(network, inputs: Dict[str, torch.Tensor], time: int, seed: Optional[int] = None, library: Optional[C.CDLL] = None) -> int:
     """Drop-in for ``network.run(inputs, time)`` of a reference ``Network`` (the body of network.py:329-465).
     ``library``: a CDLL exporting ``snn_oracle_run_window`` (CPU tensors) — default: the CUDA core on CUDA tensors."""
@@ -494,10 +537,13 @@ def run_window(network, inputs: Dict[str, torch.Tensor], time: int, seed: Option
         library.snn_oracle_run_window.argtypes = [C.POINTER(_abi.SnnNet), C.POINTER(_abi.SnnRunOpts), C.c_int, C.c_int]
         rc = library.snn_oracle_run_window(C.byref(net), C.byref(opts), 0, 0)
         del keep
+        if rc == 0:
+            _advance_averages(network, T)
         return rc | int(err.value)
     from . import _backend
 
     dev = next(iter(network.layers.values())).s.device
     _backend.run_window(net, opts, dev)
     del keep
+    _advance_averages(network, T)
     return 0

@@ -228,6 +228,30 @@ extern "C" {
                                   its [n] traces).  Also MCC_learning.MSTDPET (MCC_learning.py:652-733) on SNN_CONN_MCC, with the
                                   same fields and pointers as on SNN_CONN_DENSE */
 #define SNN_RULE_IS_MSTDP(r) ((r) == SNN_RULE_MSTDP || (r) == SNN_RULE_MSTDPET)
+/* MCC_learning.PostPre with average_update = k > 0 (MCC_learning.py:210-302): the flag is OR-ed into snn_conn_t.rule on
+ * SNN_RULE_MCC_POSTPRE of an SNN_CONN_MCC connection, whose avg_* fields (they overlay the reward-rule state) then
+ * describe the rule's averaging state, all updated in place:
+ *   avg_pre / avg_post    float32 [k, n_src, n_tgt]: average_buffer_pre / _post
+ *   avg_k                 k >= 1
+ *   avg_idx_pre / _post   average_buffer_index_pre / _post, in [0, k): the slot the next update writes
+ *   avg_continues         continues_update
+ *   avg_rows              uint32 [k, ceil(n_src / 32)]: bit i of slot q set = row i of pre slot q may be non-zero
+ *   avg_cols              uint32 [k, ceil(n_tgt / 32)]: bit j of slot q set = column j of post slot q may be non-zero
+ *                         (all zero for zero buffers; a bit may be set over a row / column of zeros)
+ * Each learning step, with U / V the step's batch-reduced terms of the plain rule without dt (s_src x fl(x_tgt * nu0) and
+ * x_src x fl(s_tgt * nu1), samples ascending from +0, / B under SNN_REDUCE_MEAN):
+ *   pre term, when nu0 != 0:  p = avg_idx_pre;  avg_pre[p] = U, avg_rows[p] = the rows with a spike in some sample;
+ *                             avg_idx_pre = (p + 1) % k;  then, when avg_continues or avg_idx_pre == 0, every (i, j) with
+ *                             row i set in some slot:  w = fl(w - fl(fl(S / k) * dt_scale)),  S = the sum of avg_pre[q][i][j]
+ *                             over the slots q with row i set, q ascending from +0 (the mean over all k slots: the others
+ *                             hold zeros, which leave such a sum as it is)
+ *   post term, when nu1 != 0: the same with avg_post, avg_cols, columns, V and w = fl(w + ...)
+ *   then decay and clamp as for the plain rule.  An element no applied term reaches keeps its value.
+ * Nothing is touched for a zero rate, and nothing in a window with learning off.  Generic tier only (tier 0 selects it;
+ * a forced tier 2 or 3 is SNN_ERR_UNSUPPORTED), no mask, and not in a plan that also holds an SNN_CONN_SPARSE connection,
+ * per-synapse tensors, per-neuron parameters or a kind of the pooling instantiation.  A library older than the flag
+ * refuses such a plan with SNN_ERR_UNSUPPORTED (it rejects every rule above SNN_RULE_MSTDPET). */
+#define SNN_RULE_AVG 0x100
 #define SNN_RULE_IS_STDP(r) (((r) >= SNN_RULE_POSTPRE && (r) <= SNN_RULE_MCC_POSTPRE) || (r) == SNN_RULE_HEBBIAN)
 
 /* ---- broadcast forms of a dense connection's per-synapse tensors (snn_conn_t wmin_t / wmax_t / nu0_t / nu1_t): which
@@ -350,11 +374,22 @@ typedef struct snn_conn {
          CONV2D: p_plus is the [B,cin,hin,win] trace image whose im2col the reference stores
                  (unfold is linear), p_minus [B,cout*hout*wout], elig [B,cout,cin*kh*kw] (fp32,
                  materialised like the reference's, applied one step later).                  */
-    float reward;      /* the run's scalar reward (network.py:319-377 -> kwargs["reward"])  */
-    float a_plus, a_minus;           /* defaults +1 / -1 (learning.py:1543-1556)            */
-    float p_plus_decay, p_minus_decay; /* exp(-dt/tc_plus), exp(-dt/tc_minus), computed by the host in fp32 */
-    float *p_plus, *p_minus, *elig;
-    uint8_t *mst_spre, *mst_spost;
+    /* SNN_RULE_MCC_POSTPRE | SNN_RULE_AVG keeps its averaging state in the same storage (see there): a connection never
+       has both rules, so the layout is the one without it. */
+    union {
+        struct {
+            float reward;      /* the run's scalar reward (network.py:319-377 -> kwargs["reward"])  */
+            float a_plus, a_minus;           /* defaults +1 / -1 (learning.py:1543-1556)            */
+            float p_plus_decay, p_minus_decay; /* exp(-dt/tc_plus), exp(-dt/tc_minus), computed by the host in fp32 */
+            float *p_plus, *p_minus, *elig;
+            uint8_t *mst_spre, *mst_spost;
+        };
+        struct {
+            float *avg_pre, *avg_post;
+            uint32_t *avg_rows, *avg_cols;
+            int32_t avg_k, avg_idx_pre, avg_idx_post, avg_continues;
+        };
+    };
     /* Network.run(..., masks={(source, target): mask}) (network.py:279-280,321,449): weights whose mask byte is non-zero are
        forced to 0 after every step's update, learning or not (AbstractConnection.update, topology.py:127-131).  [n_src, n_tgt]
        bytes, SNN_CONN_DENSE only (MulticompartmentConnection.update ignores the kwarg, topology.py:509-518); NULL = none. */

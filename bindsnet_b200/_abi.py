@@ -16,6 +16,7 @@ SNN_NODE_INPUT, SNN_NODE_LIF, SNN_NODE_DC, SNN_NODE_IF, SNN_NODE_CURRENT_LIF, SN
 SNN_NODE_SUBIF, SNN_NODE_PASSTHROUGH = 7, 8
 SNN_CONN_DENSE, SNN_CONN_MCC, SNN_CONN_CONV2D, SNN_CONN_SPARSE, SNN_CONN_MAXPOOL2D, SNN_CONN_LOCAL2D = 0, 1, 2, 3, 4, 5
 SNN_CONN_CONV3D, SNN_CONN_CONV1D, SNN_CONN_LOCAL3D, SNN_CONN_MAXPOOL3D, SNN_CONN_MEANFIELD = 6, 7, 8, 9, 10
+SNN_CONN_WNORM = 0x100
 SNN_RULE_NONE, SNN_RULE_NOOP, SNN_RULE_POSTPRE, SNN_RULE_WDEP_POSTPRE, SNN_RULE_MCC_POSTPRE, SNN_RULE_MSTDP, SNN_RULE_HEBBIAN = 0, 1, 2, 3, 4, 5, 6
 SNN_RULE_MSTDPET = 7
 SNN_RULE_AVG = 0x100
@@ -123,12 +124,18 @@ class _MeanFieldFields(C.Structure):
     _fields_ = [("mf_off", C.c_void_p), ("mf_stride", C.c_int32)]
 
 
+class _WeightNormFields(C.Structure):
+    _fields_ = [("norm_t", C.c_void_p), ("norm_step", C.c_int32)]
+
+
 class _SparseOrConv3d(C.Union):
     """The storage SNN_CONN_SPARSE's pattern, the depth axis of SNN_CONN_CONV3D / SNN_CONN_LOCAL3D /
-    SNN_CONN_MAXPOOL3D and SNN_CONN_MEANFIELD's offset map share (a connection is only one of these kinds)."""
+    SNN_CONN_MAXPOOL3D, SNN_CONN_MEANFIELD's offset map and the SNN_CONN_WNORM norm of a dense or MCC connection share
+    (a connection is only one of these kinds)."""
 
-    _anonymous_ = ("_sparse", "_conv3d", "_meanfield")
-    _fields_ = [("_sparse", _SparseFields), ("_conv3d", _Conv3dFields), ("_meanfield", _MeanFieldFields)]
+    _anonymous_ = ("_sparse", "_conv3d", "_meanfield", "_wnorm")
+    _fields_ = [("_sparse", _SparseFields), ("_conv3d", _Conv3dFields), ("_meanfield", _MeanFieldFields),
+                ("_wnorm", _WeightNormFields)]
 
 
 class _FeatureFields(C.Structure):

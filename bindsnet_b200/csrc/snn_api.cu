@@ -41,9 +41,20 @@ static int avg_check(const snn_conn_t &C) {
     return SNN_OK;
 }
 
+// A dense or MCC connection's norm tensor / per-step normalisation (snn_b200.h SNN_CONN_WNORM): the kinds that have it,
+// a norm to apply, a per-step flag on an MCC Weight only, and no averaged rule.
+static int wnorm_check(const snn_conn_t &C) {
+    const int kind = C.kind & ~SNN_CONN_WNORM;
+    if (kind != SNN_CONN_DENSE && kind != SNN_CONN_MCC) return SNN_ERR_UNSUPPORTED;
+    if (!C.has_norm || (C.norm_step != 0 && C.norm_step != 1)) return SNN_ERR_BAD_ARG;
+    if ((C.norm_step && kind != SNN_CONN_MCC) || (C.rule & SNN_RULE_AVG)) return SNN_ERR_UNSUPPORTED;
+    return SNN_OK;
+}
+
 // The plan every check and kernel below reads: the kinds without SNN_NODE_PN, pn_mask cleared on the LIF / DC layers
 // that do not carry the flag (their storage is CurrentLIFNodes' otherwise); the rules without SNN_RULE_AVG, avg_k
-// cleared on every other MCC PostPre (snn_is_avg).  *pn: some layer uses a per-neuron row.
+// cleared on every other MCC PostPre (snn_is_avg); the kinds without SNN_CONN_WNORM, norm_t / norm_step cleared on every
+// other dense or MCC connection.  *pn: some layer uses a per-neuron row.
 static int strip_pn(const snn_net_t *net, snn_net_t *out, bool *pn) {
     *pn = false;
     if (!net || net->n_layers < 0 || net->n_layers > SNN_MAX_LAYERS) return SNN_ERR_BAD_ARG;
@@ -51,6 +62,14 @@ static int strip_pn(const snn_net_t *net, snn_net_t *out, bool *pn) {
     *out = *net;
     for (int c = 0; c < net->n_conns; ++c) {
         snn_conn_t &C = out->conns[c];
+        if (C.kind & SNN_CONN_WNORM) {
+            const int rc = wnorm_check(C);
+            if (rc != SNN_OK) return rc;
+            C.kind &= ~SNN_CONN_WNORM;
+        } else if (C.kind == SNN_CONN_DENSE || C.kind == SNN_CONN_MCC) {
+            C.norm_t = nullptr;
+            C.norm_step = 0;
+        }
         if (C.rule & SNN_RULE_AVG) {
             const int rc = avg_check(C);
             if (rc != SNN_OK) return rc;
@@ -211,6 +230,15 @@ static bool has_avg(const snn_net_t *net) {
     return false;
 }
 
+// some dense or MCC connection carries a norm tensor or normalises every step (SNN_CONN_WNORM, stripped by strip_pn)
+static bool has_wn(const snn_net_t *net) {
+    for (int c = 0; c < net->n_conns; ++c) {
+        const snn_conn_t &C = net->conns[c];
+        if ((C.kind == SNN_CONN_DENSE || C.kind == SNN_CONN_MCC) && (C.norm_t || C.norm_step)) return true;
+    }
+    return false;
+}
+
 // some dense connection carries per-synapse bounds or rates (snn_b200.h)
 static bool has_syn(const snn_net_t *net) {
     for (int c = 0; c < net->n_conns; ++c)
@@ -334,6 +362,11 @@ static int select_tier(const snn_net_t *net, const snn_run_opts_t *opts, bool pn
     // snn_pool_inst_kind names, and SubtractiveResetIFNodes or PassThroughNodes), not combinations (and one for plans
     // with per-synapse bounds or rates)
     if ((int)has_sparse(net) + (int)has_feat(net) + (int)has_pool(net) + (int)has_syn(net) > 1) return 0;
+    // norm tensors / per-step normalisation: two more instantiations, alone or with features; generic tier only
+    if (has_wn(net)) {
+        if (pn || has_sparse(net) || has_pool(net) || has_syn(net) || has_avg(net)) return 0;
+        return (opts->tier == 0 || opts->tier == 1) && !opts->delta_w && !opts->delta_theta ? 1 : 0;
+    }
     // averaged MCC PostPre: two more instantiations, alone or with features; generic tier only
     if (has_avg(net)) {
         if (pn || has_sparse(net) || has_pool(net) || has_syn(net)) return 0;
@@ -374,7 +407,7 @@ size_t snn_b200_workspace_bytes(const snn_net_t *net0, const snn_run_opts_t *opt
     const snn_net_t *net = &P;
     if (validate(net, opts) != SNN_OK) return 0;
     size_t g = layout_generic(net, opts, nullptr, nullptr);
-    if (pn || has_sparse(net) || has_feat(net) || has_pool(net) || has_syn(net) || has_meanfield(net) || has_avg(net)) return g;
+    if (pn || has_sparse(net) || has_feat(net) || has_pool(net) || has_syn(net) || has_meanfield(net) || has_avg(net) || has_wn(net)) return g;
     size_t f = snn_fused_dc_supported(net, opts) ? snn_fused_dc_workspace_bytes(net, opts) : 0;
     size_t f2 = snn_fused_dc2_supported(net, opts) ? snn_fused_dc2_workspace_bytes(net, opts) : 0;
     if (f2 > f) f = f2;
@@ -420,6 +453,7 @@ int snn_b200_run_window(const snn_net_t *net0, const snn_run_opts_t *opts, void 
     }
     N.any_pool = has_pool(net) ? 1 : 0;
     N.any_avg = has_avg(net) ? 1 : 0;
+    N.any_wn = has_wn(net) ? 1 : 0;
     if (cudaMemsetAsync(N.bar, 0, sizeof(unsigned int) * SNN_BAR_ZERO_WORDS, stream) != cudaSuccess) return SNN_ERR_CUDA;
     const int e = snn_generic_launch(N, stream);
     if (e != 0) {

@@ -119,6 +119,9 @@ struct DevNet {
     float *pool_r1[SNN_MAX_CONNS];   // MaxPool2d / MaxPoo3dConnection: the workspace slot of its rates (pool_rate_slot)
     DevAvg avg[SNN_MAX_CONNS];    // MCC PostPre with averaging (snn_is_avg)
     int32_t any_avg;              // some connection is one: the plan runs an AVG instantiation
+    int32_t any_wn;               // some dense / MCC connection carries SNN_CONN_WNORM: the plan runs a WN instantiation
+    int32_t wn_units;             // per-step normalisation units of a step (a column tile of a step-normalised Weight)
+    int32_t wn_first[SNN_MAX_CONNS];   // first such unit of every connection, -1 for the others
 };
 
 // A MaxPool2dConnection's or MaxPoo3dConnection's rates, double-buffered: the gather of step t reads slot

@@ -67,7 +67,11 @@ __device__ __forceinline__ void sparse_unit(const DevNet &N, int u, int &c, int 
 // last step read a lane's own values where the other instantiations read the layer's scalars.  Combined with SYN only.
 // AVG: some MCC PostPre averages its updates (snn_b200.h SNN_RULE_AVG); only the learning phase (and the prologue's copy
 // of the slot bitmaps) differs.  Combined with FEAT only.
-template <int CTAS, bool SPARSE, bool FEAT, bool POOL, bool SYN = false, bool PN = false, bool AVG = false>
+// WN: some dense or MCC connection carries a per-target norm tensor or normalises every step (snn_b200.h
+// SNN_CONN_WNORM).  A step-normalised Weight adds one pass after the barrier that ends phases 1 / 2 (a unit per column
+// tile, as at window end) and one grid barrier behind it; its clamping rule then visits every row.  Combined with FEAT
+// only.
+template <int CTAS, bool SPARSE, bool FEAT, bool POOL, bool SYN = false, bool PN = false, bool AVG = false, bool WN = false>
 __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(const __grid_constant__ DevNet N) {
 #ifdef SNN_EMU
     float *smem = emu::tls_cta->dyn_smem;
@@ -197,6 +201,17 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
         }
         if (!grid_barrier(N.bar, G, N.err, bgen)) return;
         GPROF(3)
+        if (WN && N.wn_units) {   // Weight(norm_frequency='time step'): after the step's gather, before the rule
+            for (int u = blockIdx.x; u < N.wn_units; u += G) {
+                int c = 0;
+                #pragma unroll 1
+                for (int cc = 0; cc < N.n_conns; ++cc)
+                    if (N.wn_first[cc] >= 0 && u >= N.wn_first[cc]) c = cc;
+                const snn_conn_t &C = N.conns[c];
+                normalize_tile<true>(C, N.layers[C.src].L.n, N.layers[C.tgt].L.n, u - N.wn_first[c], M.red);
+            }
+            if (!grid_barrier(N.bar, G, N.err, bgen)) return;
+        }
         if (N.learning) {
             for (int u = blockIdx.x; u < N.p3_total; u += G) {
                 int c = 0;
@@ -212,7 +227,7 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                     const int nwS = N.layers[C.src].nw;
                     const int wg0 = (int)((long long)rc * nwS / rcn), wg1 = (int)((long long)(rc + 1) * nwS / rcn);
                     if (AVG && snn_is_avg(C)) phase3_mcc_avg(N, c, tile, wg0, wg1, t, M);
-                    else phase3<SYN>(N, c, tile, wg0, wg1, t, M);
+                    else phase3<SYN, WN>(N, c, tile, wg0, wg1, t, M);
                 }
             }
             GPROF(4)
@@ -259,7 +274,7 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
         for (int item = blockIdx.x; item < N.total_items; item += G) {
             int li, tile; item_of(N, item, li, tile);
             for (int c = 0; c < N.n_conns; ++c)
-                if (N.conns[c].tgt == li && N.conns[c].has_norm) {
+                if (N.conns[c].tgt == li && N.conns[c].has_norm && !(WN && N.conns[c].norm_step && N.conns[c].kind == SNN_CONN_MCC)) {
                     if (N.conns[c].kind == SNN_CONN_CONV2D) normalize_conv_item(N.conns[c], N.conns[c].kh * N.conns[c].kw, tile, N.layers[li].nw);
                     else if (POOL && N.conns[c].kind == SNN_CONN_CONV3D)
                         normalize_conv_item(N.conns[c], N.conns[c].kd * N.conns[c].kh * N.conns[c].kw, tile, N.layers[li].nw);
@@ -269,7 +284,7 @@ __global__ void __launch_bounds__(SNN_GEN_THREADS, CTAS) snn_generic_window(cons
                     else if (POOL && N.conns[c].kind == SNN_CONN_LOCAL3D)
                         normalize_local2d_item(N.conns[c], N.conns[c].cin * N.layers[li].L.n, N.conns[c].kd * N.conns[c].kh * N.conns[c].kw, tile,
                                              N.layers[li].nw);
-                    else normalize_tile(N.conns[c], N.layers[N.conns[c].src].L.n, N.layers[li].L.n, tile, M.red);
+                    else normalize_tile<WN>(N.conns[c], N.layers[N.conns[c].src].L.n, N.layers[li].L.n, tile, M.red);
                 }
         }
     }
@@ -316,6 +331,13 @@ static int plan_units(DevNet &N, int cap) {
         p3 += nwT * rc;
     }
     N.p3_total = p3;
+    // per-step normalisation: a unit per column tile of every such connection
+    int wnu = 0;
+    for (int c = 0; c < N.n_conns; ++c) {
+        N.wn_first[c] = -1;
+        if (N.conns[c].kind == SNN_CONN_MCC && N.conns[c].norm_step) { N.wn_first[c] = wnu; wnu += N.layers[N.conns[c].tgt].nw; }
+    }
+    N.wn_units = wnu;
     // sparse gather: (column block, chunk of SNN_GEN_WARPS samples) per SparseConnection (the blocks come from layout_generic)
     int spu = 0;
     for (int c = 0; c < N.n_conns; ++c)
@@ -327,6 +349,7 @@ static int plan_units(DevNet &N, int cap) {
     long long units = (long long)N.total_items * N.nch;
     if (p3 > units) units = p3;
     if (spu > units) units = spu;
+    if (wnu > units) units = wnu;
     bool conv_rule = false;
     for (int c = 0; c < N.n_conns; ++c)
         if (N.learning && (N.conns[c].kind == SNN_CONN_CONV2D || snn_pool_inst_kind(N.conns[c].kind)) && !snn_is_maxpool(N.conns[c].kind) &&
@@ -343,7 +366,11 @@ int snn_generic_launch(DevNet &N, cudaStream_t) {
     int sms = 3;
     if (const char *v = getenv("SNN_EMU_SMS")) sms = atoi(v) > 0 ? atoi(v) : 3;
     const int grid = plan_units(N, sms * 2);
-    if (N.any_avg && N.any_feat)
+    if (N.any_wn && N.any_feat)
+        emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, true, false, false, false, false, true>(*(const DevNet *)a); }, &N);
+    else if (N.any_wn)
+        emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, false, false, false, false, true>(*(const DevNet *)a); }, &N);
+    else if (N.any_avg && N.any_feat)
         emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, true, false, false, false, true>(*(const DevNet *)a); }, &N);
     else if (N.any_avg)
         emu::run_grid(grid, SNN_GEN_THREADS, snn_generic_smem_bytes(N.B), [](void *a) { snn_generic_window<2, false, false, false, false, false, true>(*(const DevNet *)a); }, &N);
@@ -374,8 +401,11 @@ int snn_generic_launch(DevNet &N, cudaStream_t stream) {
     const bool syn = std::any_of(N.conns, N.conns + N.n_conns, snn_has_syn);
     const bool pn = snn_dev_has_pn(N);
     bool three = false;
-    if (const char *v = getenv("SNN_B200_GVAR")) three = !sparse && !N.any_feat && !N.any_pool && !syn && !pn && !N.any_avg && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
-    const void *kern = N.any_avg ? (N.any_feat ? (const void *)snn_generic_window<2, false, true, false, false, false, true>
+    if (const char *v = getenv("SNN_B200_GVAR"))
+        three = !sparse && !N.any_feat && !N.any_pool && !syn && !pn && !N.any_avg && !N.any_wn && v[0] == '3' && 3 * (smem + 1024) <= 227 * 1024;
+    const void *kern = N.any_wn ? (N.any_feat ? (const void *)snn_generic_window<2, false, true, false, false, false, false, true>
+                                              : (const void *)snn_generic_window<2, false, false, false, false, false, false, true>)
+                     : N.any_avg ? (N.any_feat ? (const void *)snn_generic_window<2, false, true, false, false, false, true>
                                                : (const void *)snn_generic_window<2, false, false, false, false, false, true>)
                      : three ? (const void *)snn_generic_window<3, false, false, false>
                      : sparse ? (const void *)snn_generic_window<2, true, false, false>

@@ -284,9 +284,10 @@ __global__ void copy_u32_kernel(uint32_t *dst, const uint32_t *src, size_t n) {
     for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (size_t)gridDim.x * blockDim.x) dst[k] = src[k];
 }
 
+template <bool WN>
 __global__ void __launch_bounds__(SNN_GEN_THREADS) conn_normalize_kernel(snn_conn_t C, int ns, int nt) {
     SNN_SHARED(float, s_part, (SNN_NORM_CHUNKS + 1) * 32);
-    normalize_tile(C, ns, nt, blockIdx.x, s_part);
+    normalize_tile<WN>(C, ns, nt, blockIdx.x, s_part);
 }
 
 __global__ void delta_prepare_kernel(const float *__restrict__ w, const float *__restrict__ w0, float *__restrict__ dw, size_t n) {
@@ -361,8 +362,12 @@ int snn_verify_structure(const snn_conn_t &C, int n, int32_t *err, cudaStream_t 
 
 extern "C" {
 
-int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, int32_t B, const uint8_t *s, float *out,
+int snn_b200_conn_compute(const snn_conn_t *conn0, int32_t n_src, int32_t n_tgt, int32_t B, const uint8_t *s, float *out,
                           void *stream) {
+    // the product does not read the norm (SNN_CONN_WNORM: the caller normalises after it)
+    snn_conn_t K;
+    if (conn0) { K = *conn0; K.kind &= ~SNN_CONN_WNORM; }
+    const snn_conn_t *conn = conn0 ? &K : nullptr;
     if (!conn || (!conn->w && !(conn->kind == SNN_CONN_SPARSE && conn->nnz == 0) && !snn_is_maxpool(conn->kind)) || !s || !out ||
         n_src <= 0 || n_tgt <= 0 || B <= 0)
         return SNN_ERR_BAD_ARG;
@@ -441,6 +446,10 @@ int snn_b200_conn_compute(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, 
 int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *workspace, size_t workspace_bytes, void *stream_) {
     if (!net || ci < 0 || ci >= net->n_conns || B <= 0 || !workspace) return SNN_ERR_BAD_ARG;
     snn_conn_t C = net->conns[ci];
+    if (C.kind & SNN_CONN_WNORM) {   // the norm is not the rule's (a single update is a full pass: every row is clamped)
+        if (C.rule & SNN_RULE_AVG) return SNN_ERR_UNSUPPORTED;
+        C.kind &= ~SNN_CONN_WNORM;
+    }
     const bool avg = (C.rule & SNN_RULE_AVG) != 0;
     if (avg) {   // MCC PostPre with averaging (snn_b200.h): the plain rule's checks below, then its own kernel
         if (C.kind != SNN_CONN_MCC || (C.rule & ~SNN_RULE_AVG) != SNN_RULE_MCC_POSTPRE || C.mask) return SNN_ERR_UNSUPPORTED;
@@ -568,6 +577,14 @@ int snn_b200_conn_update(const snn_net_t *net, int32_t ci, int32_t B, void *work
 
 int snn_b200_conn_normalize(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt, void *stream) {
     if (!conn || n_src <= 0 || n_tgt <= 0) return SNN_ERR_BAD_ARG;
+    if (conn->kind & SNN_CONN_WNORM) {   // a norm tensor, or the per-step formula when norm_step is set (snn_b200.h)
+        const int kind = conn->kind & ~SNN_CONN_WNORM;
+        if (kind != SNN_CONN_DENSE && kind != SNN_CONN_MCC) return SNN_ERR_UNSUPPORTED;
+        if (!conn->w || (conn->norm_step != 0 && conn->norm_step != 1)) return SNN_ERR_BAD_ARG;
+        if (!conn->has_norm) return SNN_OK;
+        SNN_LAUNCH(conn_normalize_kernel<true>, (n_tgt + SNN_TILE - 1) / SNN_TILE, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, n_src, n_tgt);
+        return cuda_rc(cudaGetLastError());
+    }
     // the reference's normalize fails on a sparse w, and on a mean-field one with norm set
     if (conn->kind == SNN_CONN_SPARSE || (conn->kind == SNN_CONN_MEANFIELD && conn->has_norm)) return SNN_ERR_UNSUPPORTED;
     if (!conn->w) return SNN_ERR_BAD_ARG;
@@ -598,7 +615,7 @@ int snn_b200_conn_normalize(const snn_conn_t *conn, int32_t n_src, int32_t n_tgt
         SNN_LAUNCH(conv_normalize_kernel, (F + SNN_GEN_THREADS - 1) / SNN_GEN_THREADS, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, conn->kw);
         return cuda_rc(cudaGetLastError());
     }
-    SNN_LAUNCH(conn_normalize_kernel, (n_tgt + SNN_TILE - 1) / SNN_TILE, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, n_src, n_tgt);
+    SNN_LAUNCH(conn_normalize_kernel<false>, (n_tgt + SNN_TILE - 1) / SNN_TILE, SNN_GEN_THREADS, 0, (cudaStream_t)stream, *conn, n_src, n_tgt);
     return cuda_rc(cudaGetLastError());
 }
 

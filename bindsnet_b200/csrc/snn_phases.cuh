@@ -938,7 +938,7 @@ __device__ void phase2(const DevNet &N, int li, int tile, int chunk, int t) {
 // so that eight weight loads are in flight.
 // SYN: the connection may carry per-synapse bounds and rates (snn_b200.h wmin_t ...); plans without them run the
 // instantiation that never reads those fields.
-template <bool SYN>
+template <bool SYN, bool WN = false>
 __device__ void phase3(const DevNet &N, int ci, int tile, int wg0, int wg1, int t, const GenSmem &M) {
     const snn_conn_t &C = N.conns[ci];
     const DevLayer &S = N.layers[C.src], &G = N.layers[C.tgt];
@@ -952,7 +952,8 @@ __device__ void phase3(const DevNet &N, int ci, int tile, int wg0, int wg1, int 
     const bool wdep = C.rule == SNN_RULE_WDEP_POSTPRE || C.rule == SNN_RULE_HEBBIAN;   // plain sums: nu applied after the reduction
     const bool pre_on = stdp && C.nu0 != 0.0f, post_on = stdp && C.nu1 != 0.0f;
     const bool decay_on = C.weight_decay != 0.0f && C.weight_decay != 1.0f;
-    const bool full = decay_on || (C.has_clamp && t == 0);
+    // (WN: a connection normalised every step may leave [wmin, wmax] in any row before its update)
+    const bool full = decay_on || (C.has_clamp && (t == 0 || (WN && C.norm_step)));
     const float Bf = (float)B;
     const bool stage = pre_on && M.xt != nullptr;
     // PostPre's pre-synaptic rate of my column (per target only, snn_b200.h)
@@ -2061,6 +2062,10 @@ __device__ void mask_tile(const snn_conn_t &C, int ns, int nt, int tile) {
 
 // normalize(): Connection.normalize (topology.py:383-392) / AbstractFeature.normalize
 // (topology_features.py:250-266) on one tile; row chunking as documented in snn_b200.h.
+// WN: the connection may carry a per-target norm tensor or normalise every step (snn_b200.h SNN_CONN_WNORM); the
+// factor then follows the reference's rounding for that form, and w is read through L2, because inside a window other
+// CTAs wrote it since the last grid barrier.  Without WN the function is the scalar end-of-window normalize.
+template <bool WN = false>
 __device__ void normalize_tile(const snn_conn_t &C, int ns, int nt, int tile, float *s_part) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int j = tile * SNN_TILE + lane;
@@ -2072,7 +2077,7 @@ __device__ void normalize_tile(const snn_conn_t &C, int ns, int nt, int tile, fl
         const int i1 = min((c + 1) * chunk, ns);
         if (valid)
             for (int i = c * chunk; i < i1; ++i) {
-                const float x = C.w[(size_t)i * nt + j];
+                const float x = WN ? __ldcg(C.w + (size_t)i * nt + j) : C.w[(size_t)i * nt + j];
                 part = part + (C.norm_abs ? fabsf(x) : x);
             }
         s_part[c * 32 + lane] = part;
@@ -2082,12 +2087,15 @@ __device__ void normalize_tile(const snn_conn_t &C, int ns, int nt, int tile, fl
         float tot = 0.0f;
         for (int c = 0; c < SNN_NORM_CHUNKS; ++c) tot = tot + s_part[c * 32 + lane];
         if (tot == 0.0f) tot = 1.0f;
-        s_part[SNN_NORM_CHUNKS * 32 + lane] = C.norm / tot;
+        if (WN && C.norm_t) s_part[SNN_NORM_CHUNKS * 32 + lane] = (valid ? C.norm_t[j] : 0.0f) / tot;   // Tensor / Tensor
+        else if (WN && C.norm_step) s_part[SNN_NORM_CHUNKS * 32 + lane] = (1.0f / tot) * C.norm;   // float / Tensor
+        else s_part[SNN_NORM_CHUNKS * 32 + lane] = C.norm / tot;
     }
     __syncthreads();
     const float f = s_part[SNN_NORM_CHUNKS * 32 + lane];
     if (valid)
-        for (int i = warp; i < ns; i += SNN_GEN_WARPS) C.w[(size_t)i * nt + j] = C.w[(size_t)i * nt + j] * f;
+        for (int i = warp; i < ns; i += SNN_GEN_WARPS)
+            C.w[(size_t)i * nt + j] = (WN ? __ldcg(C.w + (size_t)i * nt + j) : C.w[(size_t)i * nt + j]) * f;
     __syncthreads();
 }
 

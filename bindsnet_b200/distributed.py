@@ -52,7 +52,15 @@ class ShardedWindowRunner:
                 if d.rule & _abi.SNN_RULE_AVG:
                     raise NotImplementedError("PostPre(average_update>0) is not supported by ShardedWindowRunner: each rank "
                                               "would average its own shard's updates, and the buffers would diverge")
+                w = conn._weight()
+                if w.norm is not None and (w.norm_frequency == "time step" or isinstance(w.norm, torch.Tensor)):
+                    raise NotImplementedError("a Weight normalised every time step or by a norm tensor is not supported by "
+                                              "ShardedWindowRunner: each rank would normalise its own replica, and the "
+                                              "combine normalises with a scalar norm at the end")
             else:
+                if getattr(conn, "_norm_tensor", lambda: None)() is not None:
+                    raise NotImplementedError("a per-target norm tensor is not supported by ShardedWindowRunner: the combine "
+                                              "normalises with a scalar norm")
                 rule = getattr(conn, "update_rule", None)
                 code = getattr(rule, "rule_code", None)
                 code = int(code) if code is not None else _abi.SNN_RULE_NONE

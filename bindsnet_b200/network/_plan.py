@@ -153,6 +153,41 @@ def fill_conn(d: "_abi.SnnConn", conn, src_idx: int, tgt_idx: int, dt: float, B:
     if d.kind == _abi.SNN_CONN_MCC:
         fill_features(d, conn)
     check_squeeze(d, conn, B)
+    if d.kind in (_abi.SNN_CONN_DENSE, _abi.SNN_CONN_MCC):
+        fill_norm(d, conn)
+
+
+def fill_norm(d: "_abi.SnnConn", conn) -> None:
+    """A per-target norm tensor or a per-step normalisation (snn_b200.h SNN_CONN_WNORM) of a dense ``Connection`` or an
+    MCC ``Weight``; other plans keep the scalar ``norm`` ``_fill_desc`` wrote."""
+    owner = conn._weight() if d.kind == _abi.SNN_CONN_MCC else conn
+    norm_t = getattr(owner, "_norm_tensor", lambda: None)()
+    step = d.kind == _abi.SNN_CONN_MCC and owner.norm_frequency == "time step"
+    if not d.has_norm or (norm_t is None and not step):
+        return
+    d.kind |= _abi.SNN_CONN_WNORM
+    d.norm_t = _ptr(norm_t) if norm_t is not None else None
+    d.norm_step = int(step)
+
+
+def norm_tensor(owner, n: int, device: torch.device) -> Optional[torch.Tensor]:
+    """``owner.norm`` as the kernels read a per-target norm: float32 ``[n]``, one value per target neuron (a ``[1, n]``
+    norm is viewed as ``[n]``).  Read in place when it lies contiguously on the weights' device, so that in-place edits
+    take effect; otherwise through a copy cached until the norm changes (``Tensor._version``)."""
+    v = owner.norm.detach()
+    if v.dim() == 2 and v.shape[0] == 1:
+        v = v[0]
+    if v.dtype != torch.float32 or tuple(v.shape) != (n,):
+        raise NotImplementedError(f"{type(owner).__name__}.norm of shape {list(owner.norm.shape)} and dtype {owner.norm.dtype}: "
+                                  f"the CUDA core scales by a float32 norm per target neuron ([{n}]) only")
+    if v.is_contiguous() and v.device == device:
+        return v
+    key = (v.data_ptr(), v._version, str(v.device), str(device))
+    cached = getattr(owner, "_b200_norm", None)
+    if cached is None or cached[0] != key:
+        cached = (key, v.to(device).contiguous(), v)
+        owner._b200_norm = cached
+    return cached[1]
 
 
 def target_bias(conn, B: int) -> Optional[torch.Tensor]:
@@ -419,7 +454,8 @@ def _conn_desc(conn, B: int, dt: float = 1.0, rule: bool = True) -> "_abi.SnnCon
 
 def compute_single_connection(conn, s: torch.Tensor, draw: Optional[Tuple[int, int, int]] = None) -> torch.Tensor:
     """``conn.compute(s)``: ``[B, *target.shape]`` currents for spikes ``s``.  ``draw`` = (seed, step, connection index)
-    of a Probability feature's draw; by default a fresh seed from torch's CPU generator, step 0, index 0."""
+    of a Probability feature's draw; by default a fresh seed from torch's CPU generator, step 0, index 0.  A 'time step'
+    Weight is normalised after the product, as its compute does (so also on the scripted tier's gather)."""
     B = s.shape[0]
     if isinstance(conn, _MaxPoolConnection):
         return _compute_pool(conn, s)
@@ -435,6 +471,8 @@ def compute_single_connection(conn, s: torch.Tensor, draw: Optional[Tuple[int, i
             draw = (int(torch.randint(0, 2**31 - 1, (1,)).item()), 0, 0)
         d.draw_seed, d.draw_step, d.draw_conn = draw[0] & 0xFFFFFFFF, draw[1] & 0xFFFFFFFF, draw[2]
     _backend.conn_compute(d, conn.source.n, conn.target.n, B, su8, out)
+    if d.kind & _abi.SNN_CONN_WNORM and d.norm_step:   # Weight.compute normalises after the product (topology_features.py:641-643)
+        conn._weight().normalize(time_step_norm=True)
     return out.view(B, *conn.target.shape)
 
 
@@ -526,11 +564,18 @@ def normalize_single_connection(conn) -> None:
     _backend.conn_normalize(d, conn.source.n, conn.target.n, conn.w.device)
 
 
-def normalize_feature(feature) -> None:
+def normalize_feature(feature, time_step: bool = False) -> None:
+    """A Weight's normalize: the window-end formula, or the per-step one when ``time_step`` (snn_b200.h SNN_CONN_WNORM)."""
     _backend.require_cuda(feature.value, "feature value")
     d = _abi.SnnConn()
     d.w = feature.value.data_ptr()
-    d.has_norm, d.norm_abs, d.norm = 1, 0, float(feature.norm)
+    d.has_norm, d.norm_abs = 1, 0
+    norm_t = feature._norm_tensor()
+    d.norm = float(feature.norm) if norm_t is None else 0.0
+    if norm_t is not None or time_step:
+        d.kind = _abi.SNN_CONN_MCC | _abi.SNN_CONN_WNORM
+        d.norm_t = _ptr(norm_t) if norm_t is not None else None
+        d.norm_step = int(time_step)
     _backend.conn_normalize(d, feature.value.shape[0], feature.value.shape[1], feature.value.device)
 
 

@@ -230,6 +230,20 @@ class Connection(AbstractConnection):
     # per-synapse wmin / wmax and learning-rate tensors run on the generic kernel (LocalConnection and SparseConnection
     # keep scalars)
     _synapse_tensors = True
+    # a norm tensor with one value per target neuron runs on the generic kernel (LocalConnection and SparseConnection
+    # keep scalars)
+    _tensor_norms = True
+
+    def _norm_tensor(self) -> Optional[torch.Tensor]:
+        """A tensor ``norm`` as float32 ``[target.n]`` (``w *= norm / |w|.sum(0)``, topology.py:383-392, a true division),
+        or None for a number.  A 0-d or one-element norm divides like the scalar path and is read as a number."""
+        if not isinstance(self.norm, torch.Tensor) or not self._tensor_norms:
+            return None
+        if self.norm.dtype == torch.float32 and tuple(self.norm.shape) in ((), (1,)):
+            return None
+        from . import _plan
+
+        return _plan.norm_tensor(self, self.target.n, self.w.device)
 
     # -- plan export -----------------------------------------------------------------------
     def _fill_desc(self, d: "_abi.SnnConn", dt: float, rule: bool = True) -> None:
@@ -241,7 +255,7 @@ class Connection(AbstractConnection):
         d.wmax = _scalar(self.wmax, "wmax") if self.wmax.numel() == 1 else np.inf
         d.has_norm = int(self.norm is not None)
         d.norm_abs = 1
-        d.norm = float(self.norm) if self.norm is not None else 0.0
+        d.norm = float(self.norm) if self.norm is not None and self._norm_tensor() is None else 0.0
         d.dt_scale = 1.0
         if rule:
             self.update_rule._fill_desc(d)
@@ -689,7 +703,7 @@ class MulticompartmentConnection(AbstractMulticompartmentConnection):
     def compute(self, s: torch.Tensor) -> torch.Tensor:
         """Reference: topology.py:437-479 + Weight.compute topology_features.py:633-645.  With a Probability feature
         every call is a new step of its own: it draws a fresh seed from torch's CPU generator, as a window without
-        ``one_spike_seed`` does."""
+        ``one_spike_seed`` does.  A 'time step' Weight normalises after the product (:641-643)."""
         from . import _plan
 
         return _plan.compute_single_connection(self, s)
@@ -780,6 +794,7 @@ class LocalConnection(Connection):
             self.norm = self.norm * kernel_prod                                    # topology.py:1437-1438
 
     _synapse_tensors = False
+    _tensor_norms = False
 
     def update(self, **kwargs) -> None:
         """topology.py:1457-1469."""
@@ -848,6 +863,7 @@ class SparseConnection(Connection):
             self.w = Parameter(self.w.to_sparse(), requires_grad=False)          # topology.py:2017
 
     _synapse_tensors = False
+    _tensor_norms = False
 
     def update(self, **kwargs) -> None:
         """topology.py:112-139 with the reference's refusal of masks on a sparse w (:129-131)."""

@@ -162,8 +162,9 @@ class Weight(AbstractFeature):
         sparse: Optional[bool] = False,
         batch_size: int = 1,
     ) -> None:
-        if norm_frequency != "sample":
-            raise NotImplementedError("Weight(norm_frequency='time step') is not implemented by the CUDA core")
+        if norm_frequency not in ("sample", "time step"):
+            raise NotImplementedError(f"Weight(norm_frequency={norm_frequency!r}) is not implemented by the CUDA core "
+                                      "(only 'sample' and 'time step')")
         if enforce_polarity:
             raise NotImplementedError("Weight(enforce_polarity=True) is not implemented by the CUDA core")
         self.norm_frequency = norm_frequency
@@ -181,16 +182,35 @@ class Weight(AbstractFeature):
             self.initialize_value = lambda: torch.rand(connection.source.n, connection.target.n)
         super().prime_feature(connection, device, enforce_polarity=self.enforce_polarity, **kwargs)
 
+    def normalize(self, time_step_norm: bool = False) -> None:
+        """topology_features.py:663-671: a 'time step' Weight normalises from its compute (``time_step_norm=True``), a
+        'sample' one from ``Network.run``'s end-of-run normalize; each call does nothing for the other frequency."""
+        if self.norm is None or time_step_norm != (self.norm_frequency == "time step"):
+            return
+        from . import _plan
+
+        _plan.normalize_feature(self, time_step=time_step_norm)
+
+    def _norm_tensor(self):
+        """The norm as float32 ``[target.n]`` (prime_feature asserted its first dimension), or None for a number."""
+        if not isinstance(self.norm, torch.Tensor):
+            return None
+        from . import _plan
+
+        return _plan.norm_tensor(self, self.value.shape[1], self.value.device)
+
     def _fill_desc(self, d: "_abi.SnnConn", dt: float, manual_update: bool) -> None:
         if self.value.dim() != 2:
             raise NotImplementedError("scalar Weight values are not supported by the CUDA core")
-        if isinstance(self.norm, torch.Tensor):
-            raise NotImplementedError("per-target tensor norms are not supported by the CUDA core yet")
+        norm_t = self._norm_tensor()
         d.has_norm = int(self.norm is not None)
         d.norm_abs = 0
-        d.norm = float(self.norm) if self.norm is not None else 0.0
+        d.norm = float(self.norm) if self.norm is not None and norm_t is None else 0.0
         d.dt_scale = float(dt)
         self.learning_rule._fill_desc(d)
+        if d.rule & _abi.SNN_RULE_AVG and self.norm is not None and (norm_t is not None or self.norm_frequency == "time step"):
+            raise NotImplementedError("PostPre(average_update>0) on a Weight normalised every time step or by a norm tensor "
+                                      "is not implemented by the CUDA core")
         if manual_update:
             d.rule = _abi.SNN_RULE_NONE
 

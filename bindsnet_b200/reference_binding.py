@@ -317,7 +317,8 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
         d.kind = _abi.SNN_CONN_MCC
         w = feat.value
         d.has_norm = int(feat.norm is not None)                                           # topology_features.py:250-266: plain sum
-        d.norm, d.norm_abs = (_f(feat.norm) if feat.norm is not None else 0.0), 0
+        d.norm, d.norm_abs = (_f(feat.norm) if feat.norm is not None and not isinstance(feat.norm, torch.Tensor) else 0.0), 0
+        norm, step = feat.norm, feat.norm_frequency == "time step"                         # :633-645, :663-671
         name = type(rule).__name__
         if name == "NoOp" or conn.manual_update:                                          # MCC_learning.py:120-146; topology.py:509-518
             d.rule = _abi.SNN_RULE_NONE
@@ -348,7 +349,10 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
                 conn.w.data = conn.w.data.contiguous()
         w = conn.w
         d.has_norm = int(conn.norm is not None)                                           # topology.py:383-392: sum of |w|
-        d.norm, d.norm_abs = (_f(conn.norm) if conn.norm is not None else 0.0), 1
+        norm, step = conn.norm, False
+        if isinstance(norm, torch.Tensor) and (type(conn).__name__ != "Connection" or tuple(norm.shape) in ((), (1,))):
+            norm = _f(norm)                                                               # one value: the scalar division
+        d.norm, d.norm_abs = (_f(norm) if norm is not None and not isinstance(norm, torch.Tensor) else 0.0), 1
         if type(conn).__name__ == "LocalConnection":
             # a dense matrix confined to its receptive fields by the connection's own mask (topology.py:1431, 1457-1469),
             # plain column sums in normalize (:1471-1479; norm is already scaled by the kernel size, :1437-1438)
@@ -400,6 +404,25 @@ def fill_connection(d: "_abi.SnnConn", conn, src: int, tgt: int, dt: float, keep
                 d.structure, d.structure_val = _abi.SNN_W_DIAG, _f(diag[0])
             elif bool(((w == w[0, 1]) | eye).all() & (diag == 0).all()):
                 d.structure, d.structure_val = _abi.SNN_W_OFFDIAG, _f(w[0, 1])
+    if d.has_norm and (isinstance(norm, torch.Tensor) or step):
+        _fill_norm(d, norm, step, int(conn.target.n), w.device, keep)
+
+
+def _fill_norm(d: "_abi.SnnConn", norm, step: bool, n: int, device, keep: List[torch.Tensor]) -> None:
+    """A per-target norm tensor (float32 [n] or [1, n]) and / or a Weight's per-step normalisation (snn_b200.h
+    SNN_CONN_WNORM)."""
+    d.kind |= _abi.SNN_CONN_WNORM
+    d.norm_step = int(step)
+    if isinstance(norm, torch.Tensor):
+        v = norm.detach()
+        if v.dim() == 2 and v.shape[0] == 1:
+            v = v[0]
+        if v.dtype != torch.float32 or tuple(v.shape) != (n,):
+            raise NotImplementedError(f"a norm of shape {list(norm.shape)} and dtype {norm.dtype}: the CUDA core scales by a "
+                                      f"float32 norm per target neuron ([{n}]) only")
+        v = v.to(device).contiguous()
+        keep.append(v)
+        d.norm_t = v.data_ptr()
 
 
 def _fill_sparse(d: "_abi.SnnConn", conn, keep: List[torch.Tensor]) -> None:

@@ -209,6 +209,26 @@ extern "C" {
                                 no mask; the target is not a PassThroughNodes layer.  Every instantiation of the generic
                                 kernel takes it; generic tier only (a forced tier 2 or 3 is SNN_ERR_UNSUPPORTED).  A
                                 library older than the kind refuses it with SNN_ERR_UNSUPPORTED */
+/* Weight normalisation with a per-target norm tensor, or after every step (MCC Weight(norm_frequency='time step'),
+ * topology_features.py:633-671).  The flag is OR-ed into snn_conn_t.kind of an SNN_CONN_DENSE or SNN_CONN_MCC
+ * connection with has_norm = 1; its norm_t / norm_step fields (they overlay the sparse storage) then describe the norm:
+ *   norm_t     NULL: the scalar `norm`; else float32 [n_tgt], norm_t[j] is target j's norm
+ *   norm_step  0: normalise at window end (normalize()), as without the flag;  1 (SNN_CONN_MCC only): normalise inside
+ *              every compute instead, and never at window end
+ * With S[j] = the column sum of w (|w| when norm_abs; summed in the SNN_NORM_CHUNKS order), S[j] == 0 -> 1:
+ *   window end, scalar norm      f = fl(norm / S)            (unchanged)
+ *   window end, norm_t           f = fl(norm_t[j] / S)       (Tensor / Tensor, topology.py:390-392, :264-266)
+ *   per step, scalar norm        f = fl(fl(1 / S) * norm)    (float / Tensor is Tensor.__rtruediv__: reciprocal * norm)
+ *   per step, norm_t             f = fl(norm_t[j] / S)
+ * then w[i, j] = fl(w[i, j] * f).  Per step (norm_abs = 0: AbstractFeature.normalize sums the signed values), step t
+ * gathers from w as step t - 1 left it, then normalises it, then the neurons update and the rule runs on the normalised
+ * w (a clamping rule clamps every element, not only those its terms reach).  This holds with learning off, under
+ * SNN_RULE_NONE and in one-step mode.  snn_b200_conn_normalize applies the formula the fields name (the per-step one
+ * after a standalone compute); snn_b200_conn_compute and _update ignore the flag.  Generic tier only (tier 0 selects it, a forced tier 2 or 3 is
+ * SNN_ERR_UNSUPPORTED); not with SNN_RULE_AVG, and not in a plan that also holds an SNN_CONN_SPARSE connection,
+ * per-synapse tensors, per-neuron parameters or a kind of the pooling instantiation.  A library older than the flag
+ * refuses such a plan with SNN_ERR_UNSUPPORTED (it rejects every kind above SNN_CONN_MEANFIELD). */
+#define SNN_CONN_WNORM 0x100
 #define SNN_RULE_NONE 0       /* MCC_learning.NoOp: update() does nothing    MCC_learning.py:120-146 */
 #define SNN_RULE_NOOP 1        /* learning.NoOp: weight decay only, no clamp  learning.py:107-146     */
 #define SNN_RULE_POSTPRE 2     /* learning.PostPre._connection_update         learning.py:390-420     */
@@ -405,7 +425,8 @@ typedef struct snn_conn {
        in place by SNN_RULE_NOOP.  A malformed pattern is reported as SNN_ERR_BAD_ARG (in *err_flag by the window).
        SNN_CONN_CONV3D (topology.py:847-1025) keeps its depth axis in the same storage: source depth din, target depth
        dout, kernel depth kd, stride sd, padding pd; SNN_CONN_MAXPOOL3D also its depth dilation dd (read by no other
-       kind).  SNN_CONN_MEANFIELD keeps its offset map and per-sample stride there.  A connection is never two of these
+       kind).  SNN_CONN_MEANFIELD keeps its offset map and per-sample stride there, and an SNN_CONN_DENSE or
+       SNN_CONN_MCC connection with SNN_CONN_WNORM its norm tensor and per-step flag.  A connection is never two of these
        kinds, so the layout is the one without them. */
     union {
         struct {
@@ -419,6 +440,10 @@ typedef struct snn_conn {
         struct {
             const int32_t *mf_off;   /* SNN_CONN_MEANFIELD: [n_tgt] element of w per target neuron (sample 0) */
             int32_t mf_stride;       /* SNN_CONN_MEANFIELD: elements of w between consecutive samples (0: shared) */
+        };
+        struct {
+            const float *norm_t;     /* SNN_CONN_WNORM: float32 [n_tgt] per-target norm, NULL = the scalar norm */
+            int32_t norm_step;       /* SNN_CONN_WNORM: 1 = normalise after every step's compute (SNN_CONN_MCC) */
         };
     };
     /* SNN_CONN_MCC with Probability / Mask / Intensity features besides its Weight (topology.py:437-479).  Each is an
